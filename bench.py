@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - the per-proof MSM + NTT kernel schedule of distributed_plonk on B200.
+"""bench.py - the per-proof MSM + NTT kernel schedule of distributed_plonk on H100.
 
 One "step" = the hot-path work of ONE TurboPlonk proof at n = 2^log_n gates exactly as the
 reference's distributed prover issues it (src/dispatcher2.rs:192-713, SURVEY.md §3.4):
@@ -17,6 +17,8 @@ metric = proofs/sec of that schedule ("prover-kernel proofs/sec": the Rust proto
   e2e   : the same schedule through the reference-facing calls with HOST buffers (pinned):
           dp_msm / dp_fft_init + dp_fft1_rows + exchange + dp_fft2, H2D and D2H inside the timing.
   roofline / cpu_baseline / clocks: see DESIGN.md §Measurement.
+
+`--dump-outputs DIR` writes what the last timed step computed (see dump_outputs).
 
 `--impl reference` times the CPU restatement of the reference path (oracle/c/ark_oracle.c, the
 arkworks algorithms incl. the per-element Fr::pow of worker.rs:79,93,113, all host cores) on a
@@ -113,6 +115,16 @@ class ClockSampler:
         busy = sorted(sm)[len(sm) // 2:]          # upper half = samples under load
         return {"sm_mhz": statistics.median(busy), "sm_max_mhz": max(mx), "power_w_max": max(power),
                 "samples": len(sm), "reasons": sorted(reasons)}
+
+
+def gpu_identity(gpu_index: int):
+    """the card a result was measured on: name and power limit (a power-capped card runs at lower clocks)"""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", str(gpu_index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1])}
+    except (OSError, subprocess.TimeoutExpired, IndexError, ValueError):
+        return {"name": None, "power_limit_w": None}
 
 
 # ------------------------------------------------------------------------------------------ CPU arm
@@ -222,6 +234,27 @@ def synthetic_k(seed: int, idx: np.ndarray) -> np.ndarray:
     return z | np.uint64(1)
 
 
+DUMP_ROWS, DUMP_SEED = 1 << 17, 0xD0_4D9   # rows sampled from an output that is larger than that
+
+
+def dump_outputs(out_dir, torch, rank, W, arrays):
+    """What the timed step's caller receives, as DIR/<name>.npy: the five 144-byte G1 commitments of the last MSM batches
+    (affine-normalised Jacobian X | Y | Z by the library) and the outputs of the last iNTT(n), coset-NTT(8n) and
+    coset-iNTT(8n) of this rank (Fr rows of 32 bytes, Montgomery form).  Every row is written as its 32-bit words in
+    float64, which holds them exactly.  An output of more than DUMP_ROWS rows is sampled: the same seeded row indices
+    every run, stored beside it as <name>_rows.npy.  At W > 1 every rank writes its own files (suffix _rank<r>)."""
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = f"_rank{rank}" if W > 1 else ""
+    for name, t in arrays.items():
+        rows = t.shape[0]
+        if rows > DUMP_ROWS:
+            idx = np.sort(np.random.default_rng(DUMP_SEED).choice(rows, DUMP_ROWS, replace=False))
+            t = t[torch.from_numpy(idx).to(t.device)]
+            np.save(os.path.join(out_dir, f"{name}_rows{sfx}.npy"), idx.astype(np.float64))
+        words = t.contiguous().cpu().numpy().view(np.uint32).reshape(t.shape[0], -1)
+        np.save(os.path.join(out_dir, f"{name}{sfx}.npy"), words.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -234,6 +267,8 @@ def main():
     ap.add_argument("--no-verify", action="store_true")
     ap.add_argument("--exchange", default="fused", choices=["fused", "nccl"],
                     help="N > 1: row kernel stores into peer memory over NVLink (fused) or one NCCL all-to-all")
+    ap.add_argument("--dump-outputs", default=None, dest="dump_outputs", metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy (float64)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference_arm(args)
@@ -310,6 +345,7 @@ def main():
         t[:, c_m // 8:, :] = 0
         in_m.append(t.view(-1, 4))
     out_m = torch.empty((cols_m * r_m, 4), dtype=torch.int64, device="cuda")
+    out_mi = torch.empty_like(out_m)      # the coset-iNTT(8n) gets its own output: both results of a step stay readable
     # what the dispatcher feeds the quotient-domain transforms is n coefficients (dispatcher2.rs:386-388): the row
     # kernels are told that columns >= c/8 of these rows are zero, as short rows tell them on the wire path (dp_fft1)
     ctx.fft_dev_hint_valid_cols(True, c_m // 8)
@@ -416,7 +452,7 @@ def main():
                 ms, nl = ctx.last_timing()
                 stats["ntt_m_ms"].append(ms)
                 stats["ntt_m_launches"] = nl
-        fft_resident(in_m[0], out_m, True, True, True, mode)
+        fft_resident(in_m[0], out_mi, True, True, True, mode)
         if record:
             section("coset_ntt_8n", t0)
 
@@ -451,6 +487,9 @@ def main():
         sampler.start()
     dt, launches = timed(step_resident, args.steps, args.warmup)
     dt_host = timed.last_host
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, torch, rank, W, {
+            "msm_commitments": torch.stack(msm_outs), "intt_n": out_n, "coset_ntt_8n": out_m, "coset_intt_8n": out_mi})
     step_resident(record=True)
     clocks = sampler.stop() if rank == 0 else None
     ms_per_step = dt / args.steps * 1e3
@@ -499,7 +538,7 @@ def main():
         # each prover round as one batch, then the transforms with two tasks of look-ahead; overlapped = a
         # commitment queued (dp_msm_submit) after every second transform.  The overlapped one is timed only if it
         # first reproduces the serial one bit for bit on this box and is not slower in a one-step trial.
-        e_steps = max(1, min(args.steps, 5))
+        e_steps = max(1, args.steps)
         try:
             step_e2e, e2e_mode = schedule.pick_schedule(
                 runner, jobs, com, ROUNDS, checksum=lambda t: int(host_of[t.out_ptr].sum()), timed=lambda f: timed(f, 1, 0, False)[0],
@@ -526,7 +565,7 @@ def main():
     if W == 1 and not args.no_e2e and os.environ.get("DP_BENCH_SKIP_RESIDENT", "0") != "1":
         try:
             from distributed_plonk_b200 import resident
-            e2e_res = resident.bench_leg(ctx, torch, log_n, rand_fr, timed, steps=max(1, min(args.steps, 3)))
+            e2e_res = resident.bench_leg(ctx, torch, log_n, rand_fr, timed, steps=max(1, args.steps))
         except Exception as e:  # the headline numbers above must survive a failure of this extra
             e2e_res = {"error": str(e)[:300]}
             ctx.sync()
@@ -581,7 +620,7 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = json.load(open(peaks_path))["hbm_gbs"], "MEASURED_PEAKS.json hbm_gbs (of measured)"
     else:
-        peak, peak_src = 6650.0, "B200_PROFILING.md fallback (of fallback)"
+        peak, peak_src = 3350.0, "NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)"
     adds, bf = schedule_units(log_n)
     msm_total = sum(stats["msm_ms"])
     acc_total = sum(stats["msm_acc_ms"])
@@ -596,21 +635,12 @@ def main():
         per_launch_ms = statistics.mean(stats["ntt_m_ms"]) / n_pass if stats["ntt_m_ms"] else float("nan")
         alg_bytes = 64 * m                                 # one read + one write of every element per pass
     achieved = alg_bytes / (per_launch_ms * 1e-3) / 1e9 if per_launch_ms == per_launch_ms else None
-    traffic = None
-    try:  # DRAM bytes per launch of the same kernel at this size, from the committed ncu capture (profiles/)
-        tr = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        key = "msm_accumulate_kernel" if dominant.startswith("msm") else "ntt_tile_kernel"
-        if W == 1:
-            ent = tr.get(key, {}).get(str(log_n) if dominant.startswith("msm") else str(log_m))
-            if ent:
-                traffic = ent["bytes"]
-    except (OSError, ValueError, KeyError):
-        pass
-    # the bound that actually applies: 32x32+64 multiply-accumulates on the FMA pipe.  Peak = plain
-    # IMAD.WIDE.U32 rate measured on this part (profiles/r01_microbench_pipes.txt: 61.9 lane-MAC/clk/SM);
-    # the carry form IMAD.WIDE.U32.X that multi-precision chains need sustains 28.3 (r01_microbench_carry_chains.txt)
-    sm_clk = (clocks or {}).get("sm_mhz") or 1965.0
-    mac_peak = 61.9 * 148 * sm_clk * 1e6
+    # the bound that actually applies: 32x32+64 multiply-accumulates on the INT32 pipe.  Peak = the 64 INT32 lanes per SM
+    # and clock of the H100 architecture (not measured) x the device's SMs x the sampled SM clock (else the 1980 MHz maximum
+    # boost clock of the H100 SXM)
+    n_sms = torch.cuda.get_device_properties(local).multi_processor_count
+    sm_clk = (clocks or {}).get("sm_mhz") or 1980.0
+    mac_peak = 64 * n_sms * sm_clk * 1e6
     tuning = ctx.msm_tuning()                                          # dp_init's choice: plain XYZZ chunks or batched-affine tree levels first
     lv = tuning["levels"]
     # Fq products per bucket addition: 10 (XYZZ mixed addition), or with L tree levels 6.4 for the (1 - 2^-L) of the additions the
@@ -619,31 +649,22 @@ def main():
     macs_msm = (hi - lo) * 1.0 * ((256 + 19) // 20) * prod_per_add * 288   # digits x Fq products x 12x12x2 MACs
     macs_ntt = (m / 2) * log_m * 128 + 4 * m * 128                     # butterflies + twiddle/coset products, 8x8x2 MACs
     compute = {
-        "bound": "int32 multiply-add pipe", "peak_mac_per_s": mac_peak, "peak_source": "measured IMAD.WIDE.U32 rate x 148 SMs x sampled SM clock",
+        "bound": "int32 multiply-add pipe", "peak_mac_per_s": mac_peak,
+        "peak_source": f"64 INT32 lanes/clk/SM (H100 architecture, not measured) x {n_sms} SMs x {sm_clk:.0f} MHz",
         "msm_accumulate_frac": (macs_msm / (statistics.mean(stats["msm_acc_ms"]) * 1e-3) / mac_peak) if stats["msm_acc_ms"] else None,
         "ntt_tile_8n_frac": (macs_ntt / (statistics.mean(stats["ntt_m_ms"]) * 1e-3) / mac_peak) if stats["ntt_m_ms"] else None,
-        "carry_form_ceiling_frac": 28.3 / 61.9,
     }
-    ntt_traffic = None
-    try:
-        ent = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json"))).get("ntt_tile_kernel", {}).get(str(log_m))
-        if W == 1 and ent:
-            ntt_traffic = ent["bytes"]
-    except (OSError, ValueError, KeyError):
-        pass
     ntt_hbm = None
     if stats["ntt_m_ms"]:
         per_tr = statistics.mean(stats["ntt_m_ms"])
         per = per_tr / n_pass
         ntt_hbm = {"kernel": "ntt_tile_kernel(8n)", "achieved": 64 * m / (per * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                    "frac": 64 * m / (per * 1e-3) / 1e9 / peak, "avg_launch_ms": per, "algorithmic_bytes_per_launch": 64 * m,
-                   "passes_per_transform": n_pass, "transform_ms": per_tr, "traffic": ntt_traffic,
+                   "passes_per_transform": n_pass, "transform_ms": per_tr,
                    # against SURVEY 8d's bytes_min = 64 N for the WHOLE transform (one read + one write of every element)
                    "per_transform_frac_of_bytes_min": 64 * m / (per_tr * 1e-3) / 1e9 / peak}
-    if lv and dominant.startswith("msm"):
-        traffic = None          # the committed ncu capture is of the plain accumulation kernel, not of the tree levels
     roofline = {"bound": "hbm", "kernel": dominant, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": (achieved / peak) if achieved else None, "traffic": traffic, "peak_source": peak_src,
+                "frac": (achieved / peak) if achieved else None, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": int(alg_bytes), "avg_launch_ms": per_launch_ms,
                 "note": "both kernels are bound by the INT32 multiply pipe, not HBM (DESIGN.md); HBM fraction reported as BASELINE asks"
                         + ("" if lv == 0 or not dominant.startswith("msm") else
@@ -657,7 +678,7 @@ def main():
         "vs_baseline": None, "dtype": "u32 limbs (255/381-bit modular integer)", "data": "synthetic",
         "config": dict(workload_config(log_n, W), exchange=exch),
         "timing": {"how": "CUDA events on the library's compute stream, max over ranks", "host_clock_ms_per_step": dt_host / args.steps * 1e3},
-        "gpu_launches": int(launches), "clocks": clocks, "verify": verify,
+        "gpu": gpu_identity(local), "gpu_launches": int(launches), "clocks": clocks, "verify": verify,
         "msm_g1_adds_per_sec": (adds / N_MSM) * (hi - lo) / nb / (statistics.mean(stats["msm_ms"]) * 1e-3) * W if stats["msm_ms"] else None,
         "ntt_butterflies_per_sec": butterflies(log_m) / (statistics.mean(stats["ntt_m_ms"]) * 1e-3) if stats["ntt_m_ms"] else None,
         "breakdown_ms": {"msm_total_one_at_a_time": msm_total, "msm_accumulate": acc_total, "intt_n_total": sum(stats["ntt_n_ms"]),

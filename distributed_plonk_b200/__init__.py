@@ -1,4 +1,4 @@
-"""distributed_plonk_b200 - B200-native (sm_100a) MSM + NTT hot path of MengLing-L/distributed_plonk.
+"""distributed_plonk_b200 - H100-native (sm_90a) MSM + NTT hot path of MengLing-L/distributed_plonk.
 
   csrc/         hand-written CUDA kernels + the C ABI (include/dplonk.h)
   _binding.py   ctypes view of the C ABI

@@ -25,7 +25,7 @@ def load() -> C.CDLL:
         path = library_path()
         if not os.path.exists(path):
             raise ExtensionMissing(
-                f"{path} not built: run `python -m distributed_plonk_b200.build` (nvcc, sm_100a). "
+                f"{path} not built: run `python -m distributed_plonk_b200.build` (nvcc, sm_90a). "
                 "distributed_plonk_b200 has no CPU or pure-Python path.")
         _cdll = bind(C.CDLL(path))
     return _cdll

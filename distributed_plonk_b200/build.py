@@ -1,4 +1,4 @@
-"""Build the CUDA library in-tree: nvcc, sm_100a only (no other arch, no CPU build)."""
+"""Build the CUDA library in-tree: nvcc, sm_90a (H100) only (no other arch, no CPU build)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "_build", "libdplonk.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 

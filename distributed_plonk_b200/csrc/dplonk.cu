@@ -130,6 +130,7 @@ struct MsmPending;  // defined with the MSM driver below
 
 struct dp_ctx {
     int device = 0;
+    uint32_t n_sms = 0;  // streaming multiprocessors of the device (sizes grids that loop over a device-side count)
     uint64_t me = 0, W = 1;
     // Three streams so that consecutive tasks overlap: rows of task k+1 stream in (s_in) while task k
     // computes (stream) and the columns of task k-1 stream out (s_out); PCIe is full duplex.
@@ -201,17 +202,15 @@ struct dp_ctx {
     uint32_t msm_affine_levels = 0;
     int msm_affine_forced = -1;             // -1 = not forced
     // env DP_MSM_TUNE: 0 = dp_init never tunes (plain pipeline unless forced); 1 (default) = msm_tune() compares the plain
-    // pipeline with two tree levels - the two pipelines that ran on a B200 before the round's GPU budget ended
-    // (profiles/r02i_msm_tuning.txt); 2 = it also tries one and three levels (what bench.py's child-process probe asks for)
+    // pipeline with two tree levels; 2 = it also tries one and three levels (what bench.py's child-process probe asks for)
     int msm_tune_mode = 1;
     uint64_t msm_affine_min_digits = (uint64_t)1 << 22;
     float tune_ms[2] = {0.f, 0.f};          // msm_tune(): plain / best candidate with levels (0 = not measured)
     float tune_all_ms[4] = {0.f, 0.f, 0.f, 0.f};  // msm_tune(): 0, 1, 2, 3 levels
     int tune_equal = -1;                    // msm_tune(): results identical (1), different (0), not run (-1)
     // knob (env DP_MSM_SORT_STREAM=1): the digit sorts of a batch run on their own stream, ahead of / under the accumulations.
-    // MEASURED AND NOT ADOPTED (profiles/r02h_ab_sort_stream.txt): 22.43 against 22.13 ms per MSM in a batch of five at 2^22 points,
-    // 3.78 against 3.76 for a 2^19-point shard - the sort's atomics and its blocks taking SM slots cost the accumulation more
-    // than the 1.0 ms (0.27 ms) of sort time that leaves the critical path.  Default: sorts queue in front of their accumulation.
+    // NOT ADOPTED (tools/ab_sort_stream.py compares the two): the sort's atomics and its blocks taking SM slots cost the
+    // accumulation more than the sort time that leaves the critical path.  Default: sorts queue in front of their accumulation.
     bool msm_sort_own_stream = false;
     int quot_table = -1;       // knob (env DP_QUOT_TABLE): -1 auto (table when it is at most 1/8 of the free memory), 0 never, 1 always
 };
@@ -1022,7 +1021,8 @@ int msm_enqueue(dp_ctx *ctx, uint64_t start, const uint4 *scalars_dev, uint64_t 
     else
         DP_LAUNCH(msm_accumulate_kernel<3>, dim3(blocks_for(max_chunks, MSM_TPB)), dim3(MSM_TPB), 0, st, offsets, g.n_keys, g.chunk, sorted,
                   bases, partials);
-    DP_LAUNCH(msm_collapse_kernel, dim3(max_multi * 32 < 148ull * 8 * MSM_TPB ? blocks_for(max_multi * 32, MSM_TPB) : 148 * 8),
+    const uint64_t collapse_cap = (uint64_t)ctx->n_sms * 8;  // one resident wave of blocks
+    DP_LAUNCH(msm_collapse_kernel, dim3(max_multi * 32 < collapse_cap * MSM_TPB ? blocks_for(max_multi * 32, MSM_TPB) : (unsigned)collapse_cap),
               dim3(MSM_TPB), 0, st, multi_keys + 1, multi_keys, (const uint32_t *)offsets_l, g.chunk, partials);
     if (record_breakdown) cudaEventRecord(ctx->ev_msm[2], st);
     DP_CUDA(ctx, cudaEventRecord(job.ev_head, st));
@@ -1330,7 +1330,7 @@ int queue_col_phase(dp_ctx *ctx, FftTask &t) {
 // =================================================================== C ABI
 extern "C" {
 
-const char *dp_version(void) { return "distributed_plonk_b200 0.1 (sm_100a)"; }
+const char *dp_version(void) { return "distributed_plonk_b200 0.1 (sm_90a)"; }
 
 const char *dp_last_error(const dp_ctx *ctx) { return ctx ? ctx->err.c_str() : g_err_noctx.c_str(); }
 
@@ -1345,9 +1345,12 @@ int dp_create(int cuda_device, uint64_t me, uint64_t n_workers, dp_ctx **out) {
     if (cuda_device < 0 || cuda_device >= n_dev) return fail(nullptr, DP_E_ARG, "dp_create: device %d of %d", cuda_device, n_dev);
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, cuda_device) != cudaSuccess) return fail(nullptr, DP_E_CUDA, "cudaGetDeviceProperties");
-    if (prop.major < 10) return fail(nullptr, DP_E_CUDA, "dp_create: device %d is sm_%d%d, need sm_100", cuda_device, prop.major, prop.minor);
+    // the library holds sm_90a code only, which runs on compute capability 9.0 and nothing else
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(nullptr, DP_E_CUDA, "dp_create: device %d is sm_%d%d, need sm_90 (H100)", cuda_device, prop.major, prop.minor);
     dp_ctx *ctx = new dp_ctx();
     ctx->device = cuda_device;
+    ctx->n_sms = (uint32_t)prop.multiProcessorCount;
     if (const char *e = getenv("DP_MSM_CHUNK")) ctx->msm_chunk = (uint32_t)atoi(e) >= 8 ? (uint32_t)atoi(e) : 0;
     if (const char *e = getenv("DP_NTT_BLOCKS")) ctx->ntt_min_blocks = atoi(e) == 2 ? 2 : 3;
     if (const char *e = getenv("DP_NTT_PREFETCH")) ctx->ntt_tw_prefetch = atoi(e) != 0;

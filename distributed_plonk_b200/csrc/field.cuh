@@ -307,9 +307,9 @@ struct Field : Limbs<P::N> {
 #if defined(__CUDACC__)
     __device__ __noinline__ static Field sqr_outlined(Field a) { return sqr_inline(a); }
 #endif
-    // MEASURED AND NOT ADOPTED (profiles/r02c_msm_shard_profile.txt): ptxas splits the single-result multiply-adds
-    // with carry into IMAD + IADD3.X pairs, the additions land on the ALU pipe next to the carry work that is already
-    // there, and msm_accumulate got 5 % SLOWER (20.2 against 19.3 ms) although 13 % of its multiplier work is gone.
+    // NOT ADOPTED: ptxas splits the single-result multiply-adds with carry into IMAD + IADD3.X pairs, the additions land
+    // on the ALU pipe next to the carry work that is already there, and msm_accumulate got slower although 13 % of its
+    // multiplier work is gone.
     // sqr() therefore stays the general product; sqr_inline() is kept, tested bit for bit (tests/test_emul_field.py).
     DP_HD Field sqr() const {
         if (P::DEDICATED_SQR) {
@@ -375,8 +375,8 @@ struct Field : Limbs<P::N> {
     }
     // 1/x for ONE thread on the critical path (msm_final: a single lane normalises the result): binary extended
     // Euclid on the limbs - shifts, additions and comparisons only, ~1.5 * bits iterations with data-dependent
-    // branches - instead of the ~1.5 * bits dependent Montgomery products of Fermat's exponentiation (0.7 ms for a
-    // lone warp at Fq size, ncu r02; this is ~10x shorter).  Divergent across a warp: keep inverse() for full warps.
+    // branches - instead of the ~1.5 * bits dependent Montgomery products of Fermat's exponentiation (a long
+    // serial chain for a lone warp at Fq size; this is ~10x shorter).  Divergent across a warp: keep inverse() for full warps.
     // x != 0, Montgomery form in and out.
     DP_HD Field inverse_vartime() const {
         uint32_t u[N], v[N], x1[N], x2[N];

@@ -1,4 +1,4 @@
-// Pippenger-bucket multi-scalar multiplication over BLS12-381 G1 for sm_100a.
+// Pippenger-bucket multi-scalar multiplication over BLS12-381 G1 for sm_90a.
 //
 // Replaces ark-ec 0.3.0 VariableBaseMSM::multi_scalar_mul as called by the reference worker
 // (src/worker.rs:117-123 commit_polynomial, 159-185 var_msm; twin call sites
@@ -27,7 +27,7 @@
 //
 // Work: N*ceil(256/c) mixed additions (10 Fq mul) dominate; HBM traffic is ~96 B gathered per
 // addition plus 32 B per scalar per pass - the kernel set is bound by the INT32 multiply pipe,
-// not by HBM (see DESIGN.md for the roofline numbers).
+// not by HBM (DESIGN.md).
 #pragma once
 #include "g1.cuh"
 #include "rt.cuh"
@@ -74,7 +74,7 @@ inline MsmGeom msm_make_geom(uint32_t c, bool pre, uint64_t stride) {
     g.n_keys = g.red_windows * g.bpw;
     // buckets per reduce thread: 16 while the bucket set is large (throughput-bound: 3.4 point operations per bucket);
     // small sets - a worker's shard of a multi-GPU MSM gets a narrower window - are latency-bound (a thread's chain of
-    // 2*seg additions + a ~1.5*log2(buckets/seg)-step scalar multiple: 2.0 ms for 2^15 buckets at seg 16, ncu r02), so
+    // 2*seg additions + a ~1.5*log2(buckets/seg)-step scalar multiple), so
     // they get more, shorter threads
     uint32_t seg = g.bpw >= (1u << 18) ? 16 : g.bpw >= (1u << 17) ? 8 : g.bpw >= (1u << 16) ? 4 : 2;
     if (seg > MSM_SEG) seg = MSM_SEG;
@@ -458,8 +458,7 @@ __global__ void __launch_bounds__(MSM_TPB, MINB) msm_accumulate_kernel(const uin
 // Before the XYZZ chunks, L levels of a pairwise tree inside every bucket: level l replaces the elements (2k, 2k+1) of
 // the bucket-ordered sequence by their sum, an AFFINE addition whose field inversion is shared by a whole thread block
 // (Montgomery's trick): 6.4 field products per addition at 16 pairs per thread against 10 for the XYZZ mixed addition
-// (measured per level on B200, tools/microbench6.cu -> profiles/r02h_microbench_affine2.txt: 0.83x the time on gathered
-// operands, 0.79x on contiguous ones).  For pairs never to straddle two buckets every bucket's slice of the sorted index
+// (tools/microbench6.cu times one level of each).  For pairs never to straddle two buckets every bucket's slice of the sorted index
 // array is padded to a multiple of 2^L entries (msm_pad_counts_kernel; the holes keep the 0xffffffff the array was
 // filled with = the point at infinity), so all levels are plain strided passes and bucket b's survivors sit at
 // offsets[b] >> L afterwards.  One level = three kernels:

@@ -1,4 +1,4 @@
-// NTT / iNTT over BLS12-381 Fr for sm_100a.
+// NTT / iNTT over BLS12-381 Fr for sm_90a.
 //
 // Replaces ark-poly 0.3.0 Radix2EvaluationDomain::{fft,ifft}_in_place and the per-element
 // Fr::pow coset / twiddle loops around it in the reference worker:
@@ -248,7 +248,7 @@ __global__ void __launch_bounds__(NTT_TPB, MINB) ntt_tile_kernel(NttPass p) {
 
     // ---- the omega_N twiddles of the epilogue are known now: optionally pull them towards L2 while the tile is loaded
     // and transformed (the table of a 2^25-point domain is 512 MiB; a demand miss in the store loop costs ~1 us).
-    // Measured on B200 (profiles/README.md): DRAM reads of the 2-D twiddle pass grow from 4.3 to 6.8 GB - off by default.
+    // Off by default: the prefetches add DRAM reads of their own to the 2-D twiddle pass.
     if (p.tw_tab && p.tw_prefetch) {
         const uint64_t n_tw = (uint64_t)1 << p.tw_log_n, half_tw = n_tw >> 1;
         for (uint32_t idx = tid; idx < tile; idx += NTT_TPB) {

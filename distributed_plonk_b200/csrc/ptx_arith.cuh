@@ -3,7 +3,7 @@
 // On the device every primitive is ONE PTX instruction that reads and/or writes the PTX
 // condition-code register (add.cc / addc / mad.lo.cc / madc.hi.cc ...).  ptxas keeps the CC
 // dependency between consecutive `asm volatile` statements, fuses mad.lo/mad.hi pairs into
-// IMAD.WIDE.U32 and turns the chains into IADD3.X / IMAD.WIDE.U32.X on sm_100a.
+// IMAD.WIDE.U32 and turns the chains into IADD3.X / IMAD.WIDE.U32.X on sm_90a.
 //
 // On the host (g++ or nvcc's host pass) the same functions are emulated with an explicit
 // carry flag, so the multi-precision algorithms in field.cuh / g1.cuh can be unit-tested
@@ -92,7 +92,7 @@ DP_HD uint32_t madc_hi(uint32_t a, uint32_t b, uint32_t c) {
 }
 
 // ---- fused lo/hi pairs: one asm statement per 32x32->64 multiply-accumulate so that ptxas
-// emits a single IMAD.WIDE.U32(.X) for it (verified with cuobjdump -sass on sm_100a).
+// emits a single IMAD.WIDE.U32(.X) for it (verified with cuobjdump -sass on sm_90a).
 // {hi:lo} = a*b
 DP_HD void mul_wide(uint32_t &lo, uint32_t &hi, uint32_t a, uint32_t b) {
     asm("mul.lo.u32 %0, %2, %3; mul.hi.u32 %1, %2, %3;" : "=r"(lo), "=r"(hi) : "r"(a), "r"(b));

@@ -67,7 +67,7 @@ __global__ void fr_invert_kernel(Fr *x, uint64_t n) {
 // ------------------------------------------------------------------ round 3: quotient evaluations
 // The quotient kernel is ~60 field multiplications of straight-line code per thread; inlined that is
 // > 120 KB of instructions streamed through the instruction cache by every warp.  Calling the
-// out-of-line multiplication keeps the kernel a few KB (the lesson of msm_reduce: 215 ms -> 1.4 ms).
+// out-of-line multiplication keeps the kernel a few KB (the lesson of msm_reduce, which ran two orders of magnitude slower inlined).
 DP_D Fr qmul(const Fr &a, const Fr &b) {
 #if defined(__CUDA_ARCH__)
     return Fr::mul_outlined(a, b);

@@ -8,7 +8,7 @@
 #define DP_DYN_SMEM(name) unsigned char *name = dp_emul::t_dyn_smem
 #else
 #if !defined(__CUDACC__)
-#error "distributed_plonk_b200 is a CUDA library: compile with nvcc for sm_100a (no CPU build exists)"
+#error "distributed_plonk_b200 is a CUDA library: compile with nvcc for sm_90a (no CPU build exists)"
 #endif
 #include <cuda_runtime.h>
 #define DP_LAUNCH(kernel, grid, block, smem, stream, ...) kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)

@@ -1,5 +1,5 @@
 /*
- * dplonk.h - C ABI of the B200-native worker hot path of MengLing-L/distributed_plonk.
+ * dplonk.h - C ABI of the H100-native worker hot path of MengLing-L/distributed_plonk.
  *
  * The reference worker (Rust) has no FFI today: its RPC method bodies call arkworks directly
  * (SURVEY.md §8b).  Each entry point below is what the body of one `PlonkSlave` / `PlonkPeer`
@@ -21,7 +21,7 @@
  * unchanged until dp_fft2 of that task (or dp_sync) returns; ordinary pageable memory - what a
  * Cap'n Proto message gives the reference worker - is staged before the call returns.  A context is bound to one CUDA device and must be used from one thread
  * at a time (the reference worker is single-threaded: worker.rs:441,453).  There is no CPU
- * fallback: dp_create fails with DP_E_CUDA when no sm_100 device is usable.
+ * fallback: dp_create fails with DP_E_CUDA when no sm_90 (H100) device is usable.
  */
 #ifndef DPLONK_H
 #define DPLONK_H

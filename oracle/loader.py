@@ -12,34 +12,21 @@ _SO = os.path.join(_HERE, "_build", "libark_oracle.so")
 _lib = None
 
 
-def _cpu_tag() -> str:
-    try:
-        with open("/proc/cpuinfo") as f:
-            for line in f:
-                if line.startswith("model name"):
-                    return line.split(":", 1)[1].strip()
-    except OSError:
-        pass
-    return "unknown"
-
-
 def build(force: bool = False) -> str:
-    """(Re)build with -march=native; rebuilt when the source is newer or the host CPU changed
-    (the .so travels to the GPU box with the repo snapshot)."""
+    """(Re)build when missing or older than its source.  The flags are portable (oracle/Makefile), so a library built on
+    one host runs on another and a tree that was built once - possibly read-only by then - is never written again."""
     src = os.path.join(_HERE, "c", "ark_oracle.c")
-    stamp = os.path.join(_HERE, "_build", "host.txt")
-    tag = _cpu_tag()
-    same_host = os.path.exists(stamp) and open(stamp).read() == tag
-    if force or not same_host or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(src):
+
+    def stale():
+        return force or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(src)
+
+    if stale():
         import fcntl
         os.makedirs(os.path.dirname(_SO), exist_ok=True)
         with open(_SO + ".lock", "w") as lock:      # several processes of one test may get here together
             fcntl.flock(lock, fcntl.LOCK_EX)
-            same_host = os.path.exists(stamp) and open(stamp).read() == tag
-            if force or not same_host or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(src):
+            if stale():
                 subprocess.check_call(["make", "-s", "-B", "-C", _HERE])
-                with open(stamp, "w") as f:
-                    f.write(tag)
     return _SO
 
 

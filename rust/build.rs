@@ -3,7 +3,7 @@
 //   DPLONK_ROOT=/path/to/this/repo cargo build --release --bin worker_gpu
 //
 // libdplonk.so is produced by `python -m distributed_plonk_b200.build`
-// (nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared; the CUDA runtime is linked statically into it,
+// (nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared; the CUDA runtime is linked statically into it,
 // so the Rust side needs no CUDA toolkit).  NCCL is only needed by worker_gpu's optional `nccl` feature (the
 // fused peer-memory exchange of dp_peer_* needs nothing but the library).
 fn main() {

@@ -306,7 +306,8 @@ inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) {
     p->multiProcessorCount = 4;
     p->totalGlobalMem = (size_t)8 << 30;
     snprintf(p->name, sizeof p->name, "cpu-emulator");
-    p->major = 10;
+    p->major = 9;
+    p->minor = 0;
     return cudaSuccess;
 }
 inline cudaError_t cudaMalloc(void **p, size_t n) {

@@ -1,7 +1,6 @@
 """The batched-affine MSM levels (DP_MSM_AFFINE / DP_MSM_TUNE) on the GPU.  Last file of the suite on purpose: these
-kernels were written after the round's GPU budget was spent (their inner loops ran on hardware in microbenchmark form
-and, as dp_init's default tuning at 2^20 and 2^22 points, with the round's last GPU seconds: profiles/r02i_msm_tuning.txt),
-so nothing else in the suite runs after the forced-level cases and the wider search exercised here."""
+kernels are the newest of the library, so nothing else in the suite runs after the forced-level cases and the wider
+search exercised here."""
 import os
 
 import numpy as np

@@ -1,9 +1,8 @@
 // EXPERIMENT: Montgomery multiplication in BLS12-381 Fr / Fq on the FP64 pipe (DFMA), 52-bit limbs.
 //
-// Why: the 32-bit carry-chain product of field.cuh is bound by IMAD.WIDE.U32.X, which issues at half
-// rate on B200 (profiles/r01_microbench_carry_chains.txt: 28 lane-MAC/clk/SM): 128 of them per Fr
-// product = 4.6 SM-cycles per product.  B200 keeps a full-rate FP64 pipe that the prover never
-// touches.  A double holds a 52-bit limb exactly, and two fused multiply-adds with round-to-zero
+// Why: the 32-bit carry-chain product of field.cuh is bound by IMAD.WIDE.U32.X, which issues at a
+// lower rate than the plain form: 128 of them per Fr product.  The FP64 pipe (on H100 at half the
+// FP32 rate) is otherwise untouched by the prover.  A double holds a 52-bit limb exactly, and two fused multiply-adds with round-to-zero
 // split an exact 104-bit limb product into its high and low 52 bits:
 //      hi = fma_rz(a, b, 2^104)            = 2^104 + floor(a*b / 2^52) * 2^52
 //      lo = fma_rz(a, b, 2^104 + 2^52 - hi) = 2^52  + (a*b mod 2^52)

@@ -1,13 +1,12 @@
 // EXPERIMENT (negative result, not part of the product): carry-free ("unsaturated limb") Montgomery
-// arithmetic.  Measured on B200 (profiles/r01_microbench_unsaturated.txt): Fr 39 G mul/s against
-// 58 G/s for the carry-chain form of field.cuh, Fq 18 against 30 - the extra partial products and
-// the 64-bit accumulator register traffic cost more than the half-rate carry forms save.
+// arithmetic.  It was measured slower than the carry-chain form of field.cuh (tools/microbench5.cu
+// times both) - the extra partial products and the 64-bit accumulator register traffic cost more
+// than the slower carry forms save.
 //
 // Carry-free ("unsaturated limb") Montgomery arithmetic.
 //
-// Why: on B200 the carry forms of the integer multiply-add are half rate - measured
-// IMAD.WIDE.U32 62 lane-MAC/clk/SM against IMAD.WIDE.U32.X 28 (profiles/r01_microbench_*.txt) - so
-// the classic 32-bit-limb Montgomery product of field.cuh, which is one long carry chain per row,
+// Why: the carry forms of the integer multiply-add (IMAD.WIDE.U32.X) issue at a lower rate than the
+// plain IMAD.WIDE.U32 (tools/microbench.cu measures both) - so the classic 32-bit-limb Montgomery product of field.cuh, which is one long carry chain per row,
 // runs at less than half of the multiplier's throughput.  Here a field element is L limbs of
 // W < 32 bits held in 32-bit registers; partial products are accumulated in 64-bit columns with
 // plain IMAD.WIDE.U32 (no carry in or out: W is chosen so that a column never overflows 64 bits)

@@ -1,5 +1,5 @@
 // Pipe-throughput microbenchmarks on the real part (exploratory; numbers quoted in DESIGN.md).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/microbench tools/microbench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/microbench tools/microbench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "../distributed_plonk_b200/csrc/g1.cuh"

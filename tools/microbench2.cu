@@ -1,5 +1,5 @@
 // Carry-chain throughput: is IMAD.WIDE.U32.X (carry-in/out) slower than plain IMAD.WIDE.U32 ?
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/microbench2 tools/microbench2.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/microbench2 tools/microbench2.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <stdint.h>

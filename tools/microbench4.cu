@@ -1,5 +1,5 @@
 // Feasibility microbenchmark for batched-affine bucket accumulation (DESIGN.md §7, planned for round 2).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -o tools/microbench4 tools/microbench4.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -o tools/microbench4 tools/microbench4.cu
 //   ./tools/microbench4 [log2 pairs, default 24]
 //
 // One tree level of a batched-affine reduction = M independent affine additions P_k + Q_k sharing field

@@ -1,5 +1,5 @@
 // FP64-pipe field multiplication (tools/experiments/dfield.cuh) against the 32-bit carry-chain product.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -o tools/microbench5 tools/microbench5.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -o tools/microbench5 tools/microbench5.cu
 // Prints: raw DFMA rate; the hi/lo split mix (2 DFMA + DADD + 64-bit integer adds); Fr / Fq Montgomery
 // products per second on the FP64 pipe, on the integer pipe, and with both kinds of warps resident
 // together (do the pipes overlap?); a bit-for-bit check of the FP64 product against field.cuh.

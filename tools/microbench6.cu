@@ -1,6 +1,6 @@
 // Batched-affine tree level, second attempt (DESIGN.md section 7): serial prefix products per thread instead of a
 // product tree over single pairs.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -o tools/microbench6 tools/microbench6.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -o tools/microbench6 tools/microbench6.cu
 //   ./tools/microbench6 [log2 pairs, default 24]
 // tools/microbench4.cu (round 2) measured one level of P_k + Q_k with a 256-leaf product tree over 2 pairs per thread:
 // 1.69x SLOWER than the XYZZ mixed addition, because the tree levels run with mostly idle warps (36 warp-products per
