@@ -18,6 +18,7 @@ EXPORTS = [
     "dp_poly_div_linear", "dp_poly_div_linear_dev", "dp_init_compressed", "dp_get_bases",
     "dp_msm_submit", "dp_msm_collect", "dp_poly_put", "dp_poly_ptr", "dp_poly_get", "dp_poly_free", "dp_commit_dev",
     "dp_fft_exchange_begin_async", "dp_compute_stream", "dp_fft_dev_p2p_async", "dp_fft1_rows_short", "dp_fft_dev_hint_valid_cols", "dp_ntt_dev_padded", "dp_debug_set_three_pass",
+    "dp_ntt_dev_quot_slice", "dp_quotient_evals_slice_dev",
 ]
 
 
@@ -98,6 +99,8 @@ def bind(cdll: C.CDLL) -> C.CDLL:
         "dp_get_bases": (i, [vp, u64, sz, vp]),
         "dp_quotient_evals": (i, [vp, C.POINTER(QuotientArgs), vp]),
         "dp_quotient_evals_dev": (i, [vp, C.POINTER(QuotientArgs), vp]),
+        "dp_quotient_evals_slice_dev": (i, [vp, C.POINTER(QuotientArgs), u32, vp]),
+        "dp_ntt_dev_quot_slice": (i, [vp, vp, sz, u32, vp, i]),
         "dp_poly_eval": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_eval_dev": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_lincomb": (i, [vp, C.POINTER(vp), C.POINTER(sz), vp, sz, vp, sz]),
@@ -327,6 +330,13 @@ class Context:
         q = self._quotient_args(selectors, sigmas, wires, perm, pub_input, k, alpha, beta, gamma, keep)
         self._ck(self.lib.dp_quotient_evals_dev(self.h, C.byref(q), out_ptr))
 
+    def quotient_evals_slice_dev(self, selectors, sigmas, wires, perm, pub_input, k, alpha, beta, gamma, slice_: int, out_ptr: int):
+        """round 3 for slice `slice_` of the quotient coset: the 25 arrays hold n points each (ntt_dev_quot_slice); writes
+        out[slice_ + (m/n) i], i < n, of the m-point output"""
+        keep = []
+        q = self._quotient_args(selectors, sigmas, wires, perm, pub_input, k, alpha, beta, gamma, keep)
+        self._ck(self.lib.dp_quotient_evals_slice_dev(self.h, C.byref(q), slice_, out_ptr))
+
     def poly_eval(self, coeffs, point: np.ndarray, n: int | None = None) -> np.ndarray:
         """round 4: p(point); coeffs = [n,4] host array, or a device pointer with n given"""
         pt, out = np.ascontiguousarray(point, dtype=np.uint64), np.empty(4, dtype=np.uint64)
@@ -403,6 +413,11 @@ class Context:
     def ntt_dev_padded(self, data_ptr: int, n_valid: int, log_n: int, is_inv: bool, is_coset: bool, wait: bool = True):
         """in place on 2^log_n Fr at data_ptr whose entries from n_valid on are zero"""
         self._ck(self.lib.dp_ntt_dev_padded(self.h, data_ptr, n_valid, log_n, int(is_inv), int(is_coset), int(wait)))
+
+    def ntt_dev_quot_slice(self, coeffs_ptr: int, n_valid: int, slice_: int, out_ptr: int, wait: bool = True):
+        """p(s * omega_n^i), i < n, s = g * omega_m^slice_: slice slice_ of the coset evaluation on the quotient domain, of the
+        n_valid coefficients at coeffs_ptr (only read), into the n Fr at out_ptr"""
+        self._ck(self.lib.dp_ntt_dev_quot_slice(self.h, coeffs_ptr, n_valid, slice_, out_ptr, int(wait)))
 
     def fft_dev(self, rows_ptr: int, cols_ptr: int, is_quot: bool, is_inv: bool, is_coset: bool):
         self._ck(self.lib.dp_fft_dev(self.h, rows_ptr, cols_ptr, int(is_quot), int(is_inv), int(is_coset)))

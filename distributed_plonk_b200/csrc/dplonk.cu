@@ -101,6 +101,9 @@ struct DomainDev {
     // plan_whole_ntt uses; two small table reads and two products instead of one Fr::pow per element
     Fr *wg_a = nullptr, *wg_b = nullptr, *wgi_a = nullptr, *wgi_b = nullptr;
     uint32_t w_l1 = 0, w_ll = 0;
+    // gate domain only: the same pair for each slice shift s_k = g * omega_m^k, k < m/n (the quotient domain's slices,
+    // dp_ntt_dev_quot_slice): ws_a[k * 2^(L-l1) + j] = s_k^j, ws_b[k * 2^l1 + j] = s_k^(2^(L-l1) * j)
+    Fr *ws_a = nullptr, *ws_b = nullptr;
     uint64_t n() const { return (uint64_t)1 << log_n; }
     uint64_t r() const { return (uint64_t)1 << log_r; }
     uint64_t c() const { return (uint64_t)1 << log_c; }
@@ -646,19 +649,37 @@ int whole_split(const dp_ctx *ctx, uint32_t L, uint32_t l[3]) {
     return 3;
 }
 
+// The factor tables of domain d serve a whole-domain transform of 2^L points when they were built for its pass split
+bool whole_tables_fit(const dp_ctx *ctx, const DomainDev *d, uint32_t L) {
+    uint32_t l[3];
+    const int np = whole_split(ctx, L, l);
+    return d && d->log_n == L && d->wg_a && np >= 2 && d->w_l1 == l[0] && d->w_ll == l[np - 1];
+}
+
+// Forward coset factors of a whole-domain transform that replace the domain's own wg_a / wg_b (a shift other than g)
+struct CosetTables {
+    const Fr *a, *b;
+};
+
 // Whole-domain transform of 2^L elements: x (in place) with scratch of the same size.  n_valid: x[n_valid..) is
 // zero (a coefficient vector shorter than the domain): the first pass then reads and multiplies only what is there.
+// src != nullptr: out of place, the first pass reads src instead of x (src is never written; only its first n_valid
+// entries are read when the first pass's zero-input cut falls exactly on n_valid - the caller checks, see slice_ntt_device).
+// shift != nullptr: forward coset with those factor tables instead of the domain's (requires whole_tables_fit).
 int plan_whole_ntt(dp_ctx *ctx, const DomainDev *d, Fr *x, Fr *scratch, uint32_t L, bool is_inv, bool is_coset,
-                   const Fr *H, uint32_t H_log_n, uint64_t n_valid = 0) {
+                   const Fr *H, uint32_t H_log_n, uint64_t n_valid = 0, const Fr *src = nullptr, const CosetTables *shift = nullptr) {
     const uint64_t N = (uint64_t)1 << L;
     if (n_valid == 0 || n_valid > N) n_valid = N;
     uint32_t l[3];
     const int np = whole_split(ctx, L, l);
     if (np == 0) return fail(ctx, DP_E_ARG, "dp_ntt: log_n %u too large for one device pass plan", L);
-    const uint32_t l1 = l[0], ll = l[np - 1];
+    const uint32_t l1 = l[0];
     Fr g = fr_from_u64(7), ninv = fr_from_u64(N).inverse();
     // coset scaling fused into the first load / the last store when this domain's factor tables fit the split
-    const bool tabs = d && d->log_n == L && d->wg_a && d->w_l1 == l1 && d->w_ll == ll && np >= 2;
+    const bool tabs = whole_tables_fit(ctx, d, L);
+    if (shift && !(tabs && is_coset && !is_inv)) return fail(ctx, DP_E_ARG, "coset factor tables do not fit the 2^%u plan", L);
+    if (src && is_coset && !tabs) return fail(ctx, DP_E_ARG, "out-of-place coset transform without factor tables");
+    const Fr *in0 = src ? src : x;
     if (is_coset && !is_inv && !tabs) {
         DP_LAUNCH(fr_scale_powers_kernel, dim3(blocks_for(n_valid, 256)), dim3(256), 0, ctx->stream, x, n_valid, g, Fr::one());
         ctx->launches++;
@@ -670,9 +691,9 @@ int plan_whole_ntt(dp_ctx *ctx, const DomainDev *d, Fr *x, Fr *scratch, uint32_t
             p.in_zlog = vlog < p.log_k ? p.log_k - vlog : 0;
         }
         if (is_coset && !is_inv && tabs) {
-            p.pre_a = d->wg_a;
+            p.pre_a = shift ? shift->a : d->wg_a;
             p.pa_l = 1;
-            p.pre_b = d->wg_b;
+            p.pre_b = shift ? shift->b : d->wg_b;
             p.pb_m = 1;
         }
     };
@@ -685,7 +706,7 @@ int plan_whole_ntt(dp_ctx *ctx, const DomainDev *d, Fr *x, Fr *scratch, uint32_t
     const uint64_t tw_mul = (uint64_t)1 << (H_log_n - L);  // omega_N = omega_H^(tw_mul)
     if (np == 1) {
         NttPass p = pass_base(ctx, is_inv);
-        p.in = x;
+        p.in = in0;
         p.out = x;
         p.log_k = L;
         p.log_g = 0;
@@ -697,7 +718,7 @@ int plan_whole_ntt(dp_ctx *ctx, const DomainDev *d, Fr *x, Fr *scratch, uint32_t
         const uint32_t l2 = l[1];
         const uint64_t N1 = (uint64_t)1 << l1, N2 = (uint64_t)1 << l2;
         NttPass p = pass_base(ctx, is_inv);
-        p.in = x;
+        p.in = in0;
         p.out = scratch;
         p.log_k = l1;
         p.log_g = pick_log_g(l1, N2);
@@ -730,7 +751,7 @@ int plan_whole_ntt(dp_ctx *ctx, const DomainDev *d, Fr *x, Fr *scratch, uint32_t
         const uint32_t l2 = l[1], l3 = l[2];
         const uint64_t N1 = (uint64_t)1 << l1, N2 = (uint64_t)1 << l2, N3 = (uint64_t)1 << l3;
         NttPass a = pass_base(ctx, is_inv);
-        a.in = x;
+        a.in = in0;
         a.out = scratch;
         a.log_k = l1;
         a.log_g = pick_log_g(l1, N2 * N3);
@@ -834,7 +855,30 @@ int build_domain(dp_ctx *ctx, DomainDev &d, uint64_t min_size) {
     return DP_OK;
 }
 
+// s_k = g * omega_m^k: the shift of slice k of the quotient coset g*H_m as cosets of the gate domain H_n,
+// g * omega_m^(k + (m/n) i) = s_k * omega_n^i
+Fr slice_shift(const DomainDev &dq, uint32_t k) { return fr_from_u64(7) * fr_domain_gen(dq.log_n).pow(k); }
+
+// the per-slice factor tables of the gate domain dg (DomainDev::ws_a / ws_b), for the m/n slices of dq; none when the
+// gate domain has no fused tables (single-pass split) or the quotient domain is not a multiple of it
+int build_slice_tables(dp_ctx *ctx, DomainDev &dg, const DomainDev &dq) {
+    if (!dg.wg_a || dq.log_n < dg.log_n || dq.log_n - dg.log_n > 4) return DP_OK;  // (ratios above RND_MAX_RATIO: no quotient)
+    const uint32_t ns = 1u << (dq.log_n - dg.log_n);
+    const uint64_t na = dg.n() >> dg.w_l1, nb = (uint64_t)1 << dg.w_l1;
+    dg.ws_a = (Fr *)ctx->pool.alloc(ns * na * sizeof(Fr));
+    dg.ws_b = (Fr *)ctx->pool.alloc(ns * nb * sizeof(Fr));
+    if (!dg.ws_a || !dg.ws_b) return fail(ctx, DP_E_OOM, "slice factor tables (%u x 2^%u)", ns, dg.log_n);
+    for (uint32_t k = 0; k < ns; k++) {
+        const Fr s = slice_shift(dq, k), one = Fr::one();
+        DP_TRY(gen_powers(ctx, dg.ws_a + k * na, na, s, 0, 1, one));
+        DP_TRY(gen_powers(ctx, dg.ws_b + k * nb, nb, s, 0, na, one));
+    }
+    return DP_OK;
+}
+
 void free_domain(dp_ctx *ctx, DomainDev &d) {
+    ctx->pool.release(d.ws_a);
+    ctx->pool.release(d.ws_b);
     ctx->pool.release(d.H);
     ctx->pool.release(d.g_row);
     ctx->pool.release(d.g_col);
@@ -1537,6 +1581,7 @@ static int init_impl(dp_ctx *ctx, const void *bases, size_t n_bases, uint64_t do
     }
     DP_TRY(build_domain(ctx, ctx->dom[0], domain_size));
     DP_TRY(build_domain(ctx, ctx->dom[1], quot_domain_size));
+    DP_TRY(build_slice_tables(ctx, ctx->dom[0], ctx->dom[1]));
     for (int k = 0; k < 2; k++) {
         const DomainDev &d = ctx->dom[k];
         if (d.r() < ctx->W || d.c() < ctx->W)
@@ -2116,6 +2161,55 @@ int dp_ntt_dev_padded(dp_ctx *ctx, void *data_dev, size_t n_valid, uint32_t log_
     return call_end(ctx, wait != 0);
 }
 
+// Slice k of the coset evaluation on the quotient domain: out[i] = p(s_k * omega_n^i), i < n, an n-point transform of the
+// gate domain with the coset shift s_k (slice_shift), out of place.  coeffs[0, n_valid) is read, never written.
+static int slice_ntt_device(dp_ctx *ctx, const Fr *coeffs, uint64_t n_valid, uint32_t k, Fr *out) {
+    const DomainDev &dg = ctx->dom[0];
+    const uint32_t L = dg.log_n;
+    const uint64_t N = dg.n();
+    const bool multi = L > ctx->max_contig_log_k;
+    Scratch tmp(ctx->pool);
+    Fr *scratch = multi ? tmp.get<Fr>(N) : nullptr;
+    if (multi && !scratch) return fail(ctx, DP_E_OOM, "dp_ntt_dev_quot_slice scratch");
+    // Fused: the first pass reads coeffs and multiplies by slice k's factor tables as it loads.  Its zero-input cut reads
+    // the leading 2^v points of each of its 2^(L - l1) lanes, which is exactly coeffs[0, n_valid) when n_valid is a power
+    // of two of at least that many lanes (the prover's n coefficients, and n/8 from 2^(3 + L - l1) on).
+    const uint64_t lanes = N >> dg.w_l1;
+    const bool exact_cut = n_valid && (n_valid & (n_valid - 1)) == 0 && n_valid >= lanes;
+    if (dg.ws_a && whole_tables_fit(ctx, &dg, L) && exact_cut) {
+        const CosetTables t{dg.ws_a + k * lanes, dg.ws_b + ((uint64_t)k << dg.w_l1)};
+        return plan_whole_ntt(ctx, &dg, out, scratch, L, false, true, dg.H, L, n_valid, coeffs, &t);
+    }
+    // otherwise (single-pass domains, a split the tables were not built for, other lengths): scale-and-copy into out,
+    // then the plain transform in place
+    DP_LAUNCH(fr_scale_powers_copy_kernel, dim3(blocks_for(N, 256)), dim3(256), 0, ctx->stream, coeffs, out, n_valid, N,
+              slice_shift(ctx->dom[1], k));
+    ctx->launches++;
+    DP_CUDA(ctx, cudaGetLastError());
+    return plan_whole_ntt(ctx, &dg, out, scratch, L, false, false, dg.H, L, n_valid);
+}
+
+static bool ranges_overlap(const void *a, uint64_t a_bytes, const void *b, uint64_t b_bytes) {
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return x < y + b_bytes && y < x + a_bytes;
+}
+
+int dp_ntt_dev_quot_slice(dp_ctx *ctx, const void *coeffs_dev, size_t n_valid, uint32_t slice, void *out_dev, int wait) {
+    if (!ctx || !coeffs_dev || !out_dev) return fail(ctx, DP_E_ARG, "dp_ntt_dev_quot_slice: NULL argument");
+    if (!ctx->inited) return fail(ctx, DP_E_STATE, "dp_ntt_dev_quot_slice before dp_init");
+    const DomainDev &dg = ctx->dom[0], &dq = ctx->dom[1];
+    const uint64_t n = dg.n();
+    if (dq.log_n < dg.log_n || slice >= (dq.n() >> dg.log_n))
+        return fail(ctx, DP_E_ARG, "dp_ntt_dev_quot_slice: slice %u of %llu", slice, (unsigned long long)(dq.log_n < dg.log_n ? 0 : dq.n() >> dg.log_n));
+    if (n_valid > n) return fail(ctx, DP_E_ARG, "dp_ntt_dev_quot_slice: %zu coefficients > n = %llu", n_valid, (unsigned long long)n);
+    if (ranges_overlap(coeffs_dev, n_valid * sizeof(Fr), out_dev, n * sizeof(Fr)))
+        return fail(ctx, DP_E_ARG, "dp_ntt_dev_quot_slice: the output overlaps the coefficients");
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    DP_TRY(slice_ntt_device(ctx, (const Fr *)coeffs_dev, n_valid, slice, (Fr *)out_dev));
+    return call_end(ctx, wait != 0);
+}
+
 int dp_ntt(dp_ctx *ctx, void *data, size_t n, uint32_t log_n, int is_inv, int is_coset) {
     if (!ctx || !data) return fail(ctx, DP_E_ARG, "dp_ntt: NULL argument");
     if (log_n > 32) return fail(ctx, DP_E_ARG, "dp_ntt: log_n %u", log_n);
@@ -2513,7 +2607,10 @@ int poly_suffix_device(dp_ctx *ctx, const Fr *in, uint64_t n, const Fr *pw, uint
     return DP_OK;
 }
 
-int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arrays /* 25 device arrays */, Fr *out_dev) {
+// slice < 0: the whole quotient coset (25 arrays of m points); else slice k of it (25 arrays of n points, DESIGN.md 3.4):
+// points g * omega_m^(k + (m/n) i), written to out_dev[k + (m/n) i]
+int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arrays /* 25 device arrays */, Fr *out_dev,
+                    int slice = -1) {
     const DomainDev &dq = ctx->dom[1], &dg = ctx->dom[0];
     const uint64_t m = dq.n(), n = dg.n();
     if (m < n || m / n > RND_MAX_RATIO) return fail(ctx, DP_E_ARG, "quotient domain / gate domain = %llu, supported: 1..%d", (unsigned long long)(m / n), RND_MAX_RATIO);
@@ -2542,12 +2639,18 @@ int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arr
         cur = cur * wn;
     }
     for (uint32_t i = q.ratio; i < RND_MAX_RATIO; i++) q.zh_inv[i] = Fr::zero();
+    if (slice >= (int)q.ratio) return fail(ctx, DP_E_ARG, "quotient slice %d of %u", slice, q.ratio);
     q.H = dq.H;
     q.m = m;
     q.log_m = dq.log_n;
     q.out = out_dev;
+    const QuotPts pts = slice < 0 ? QuotPts{m, 0, 1} : QuotPts{n, (uint32_t)slice, q.ratio};
+    q.pts = pts.pts;
+    q.first = pts.first;
+    q.step = pts.step;
+    q.z_next = slice < 0 ? q.ratio : 1;   // z(omega x): omega_n = omega_m^ratio, one step within a slice
     // all blocks' 1 / prod(x_i - 1) up front, one thread per block, instead of one serial inversion inside each block
-    const unsigned n_blocks = blocks_for(m, QUO_TPB);
+    const unsigned n_blocks = blocks_for(pts.pts, QUO_TPB), m_blocks = blocks_for(m, QUO_TPB);
     Scratch tmp(ctx->pool);
     // the 1/(x_i - 1) are the same for every proof on this domain: keep them when the table fits
     bool want_table = ctx->quot_table == 1;
@@ -2559,12 +2662,12 @@ int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arr
     if (want_table && !(ctx->quot_inv && ctx->quot_inv_log == dq.log_n)) {
         ctx->pool.release(ctx->quot_inv);
         ctx->quot_inv = (Fr *)ctx->pool.alloc(m * sizeof(Fr));
-        if (ctx->quot_inv) {
-            Fr *prod = tmp.get<Fr>(n_blocks);
+        if (ctx->quot_inv) {   // (over the whole coset, whichever points this call covers)
+            Fr *prod = tmp.get<Fr>(m_blocks);
             if (!prod) return fail(ctx, DP_E_OOM, "quotient scratch");
-            DP_LAUNCH(quotient_xm1_products_kernel, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, q.gen, q.H, q.log_m, m, prod);
-            DP_LAUNCH(fr_invert_kernel, dim3(blocks_for(n_blocks, 128)), dim3(128), 0, ctx->stream, prod, (uint64_t)n_blocks);
-            DP_LAUNCH(quotient_inv_table_kernel, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, q.gen, q.H, q.log_m, m, (const Fr *)prod,
+            DP_LAUNCH(quotient_xm1_products_kernel, dim3(m_blocks), dim3(QUO_TPB), 0, ctx->stream, q.gen, q.H, q.log_m, QuotPts{m, 0, 1}, prod);
+            DP_LAUNCH(fr_invert_kernel, dim3(blocks_for(m_blocks, 128)), dim3(128), 0, ctx->stream, prod, (uint64_t)m_blocks);
+            DP_LAUNCH(quotient_inv_table_kernel, dim3(m_blocks), dim3(QUO_TPB), 0, ctx->stream, q.gen, q.H, q.log_m, m, (const Fr *)prod,
                       ctx->quot_inv);
             ctx->launches += 3;
             ctx->quot_inv_log = dq.log_n;
@@ -2581,7 +2684,7 @@ int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arr
     } else {
         Fr *prod = tmp.get<Fr>(n_blocks);
         if (!prod) return fail(ctx, DP_E_OOM, "quotient scratch");
-        DP_LAUNCH(quotient_xm1_products_kernel, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, q.gen, q.H, q.log_m, m, prod);
+        DP_LAUNCH(quotient_xm1_products_kernel, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, q.gen, q.H, q.log_m, pts, prod);
         DP_LAUNCH(fr_invert_kernel, dim3(blocks_for(n_blocks, 128)), dim3(128), 0, ctx->stream, prod, (uint64_t)n_blocks);
         q.prod_inv = prod;
         DP_LAUNCH(quotient_kernel<false>, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, q);
@@ -2644,6 +2747,22 @@ int dp_quotient_evals_dev(dp_ctx *ctx, const dp_quotient_args *a, void *out_dev)
     const void *flat[25];
     quotient_ptrs(*a, flat);
     DP_TRY(quotient_device(ctx, *a, reinterpret_cast<const Fr *const *>(flat), (Fr *)out_dev));
+    return call_end(ctx, true);
+}
+
+int dp_quotient_evals_slice_dev(dp_ctx *ctx, const dp_quotient_args *slice_arrays, uint32_t slice, void *out_dev) {
+    DP_TRY(quotient_check(ctx, slice_arrays, out_dev, "dp_quotient_evals_slice_dev"));
+    const DomainDev &dg = ctx->dom[0], &dq = ctx->dom[1];
+    const uint64_t n = dg.n(), m = dq.n();
+    if (m < n || slice >= m / n) return fail(ctx, DP_E_ARG, "dp_quotient_evals_slice_dev: slice %u of %llu", slice, (unsigned long long)(m < n ? 0 : m / n));
+    const void *flat[25];
+    quotient_ptrs(*slice_arrays, flat);
+    for (int i = 0; i < 25; i++)
+        if (ranges_overlap(flat[i], n * sizeof(Fr), out_dev, m * sizeof(Fr)))
+            return fail(ctx, DP_E_ARG, "dp_quotient_evals_slice_dev: the output overlaps input %d", i);
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    DP_TRY(quotient_device(ctx, *slice_arrays, reinterpret_cast<const Fr *const *>(flat), (Fr *)out_dev, (int)slice));
     return call_end(ctx, true);
 }
 

@@ -471,6 +471,13 @@ __global__ void fr_scale_powers_kernel(Fr *x, uint64_t n, Fr base, Fr c) {
     gmem_st(x + i, gmem_ld(x + i) * (base.pow(i) * c));
 }
 
+// out[i] = in[i] * base^i for i < n_in, 0 for n_in <= i < n_out   (out-of-place coset scaling; `in` is not written)
+__global__ void fr_scale_powers_copy_kernel(const Fr *in, Fr *out, uint64_t n_in, uint64_t n_out, Fr base) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_out) return;
+    gmem_st(out + i, i < n_in ? gmem_ld(in + i) * base.pow(i) : Fr::zero());
+}
+
 // Montgomery -> canonical (Fr::into_repr, worker.rs:118), optionally zero-padding up to n_out
 __global__ void fr_into_repr_kernel(const Fr *in, Fr *out, uint64_t n_in, uint64_t n_out) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -5,8 +5,9 @@
 // polynomial evaluations at zeta (535-548), the linear combinations lin_poly / batch_poly (566-649)
 // and the two divisions by (X - point) that give the opening witnesses (651-690).  With the
 // polynomials resident on the worker these are four small families of kernels:
-//   * quotient_kernel        one thread per point of the quotient domain; the 1/(x_i - 1) of the
-//                            L_1 term come from ONE inversion per block (product tree in shared memory)
+//   * quotient_kernel        one thread per point of the quotient domain, or of one n-point slice of it
+//                            (DESIGN.md 3.4); the 1/(x_i - 1) of the L_1 term come from a cached table or
+//                            from ONE inversion per block (product tree in shared memory)
 //   * poly_fold_kernel       p(z): Horner per thread, tree per block, recursion over block results
 //   * poly_suffix_kernel     E_j = sum_{k>=j} p_k z^(k-j): the quotient by (X - z) is E shifted by one,
 //                            E_0 is the remainder p(z); same chunking, carries from a recursive scan
@@ -90,21 +91,32 @@ struct QuotientArgs {
     const Fr *inv_xm1;  // TABLE variant: 1 / (x_i - 1) for every point of the coset (cached per quotient domain)
     uint64_t m;
     uint32_t log_m, ratio;
+    // The points this launch covers: thread i < pts handles point pt = first + step * i of the quotient coset, reads the 25
+    // inputs at i and z(omega x) at (i + z_next) mod pts, and writes out[pt].  The whole coset: first 0, step 1, pts m,
+    // z_next = ratio.  Slice k (x = s_k omega_n^i, s_k = g omega_m^k): first k, step ratio, pts n, z_next 1.
+    uint64_t pts;
+    uint32_t first, step, z_next;
     Fr *out;
 };
 
-// x_i - 1, x_i = g * omega_m^i (lines 366-369); 1 past the end of the domain.  g*H never meets 1.
-DP_D Fr quotient_xm1(const Fr &gen, const Fr *H, uint32_t log_m, uint64_t m, uint64_t i, Fr &x) {
-    x = i < m ? gen * tw_lookup(H, i, log_m, 0) : Fr::one() + Fr::one();
+// Point set of one quotient launch (see QuotientArgs::pts)
+struct QuotPts {
+    uint64_t pts;
+    uint32_t first, step;
+};
+
+// x_i - 1, x_i = g * omega_m^(first + step * i) (lines 366-369); 1 past the end of the point set.  g*H never meets 1.
+DP_D Fr quotient_xm1(const Fr &gen, const Fr *H, uint32_t log_m, const QuotPts &s, uint64_t i, Fr &x) {
+    x = i < s.pts ? gen * tw_lookup(H, s.first + (uint64_t)s.step * i, log_m, 0) : Fr::one() + Fr::one();
     return x - Fr::one();
 }
 
 // pre-pass: prod[b] = product of (x_i - 1) over the points of quotient block b
-__global__ void __launch_bounds__(QUO_TPB) quotient_xm1_products_kernel(Fr gen, const Fr *H, uint32_t log_m, uint64_t m, Fr *prod) {
+__global__ void __launch_bounds__(QUO_TPB) quotient_xm1_products_kernel(Fr gen, const Fr *H, uint32_t log_m, QuotPts ps, Fr *prod) {
     __shared__ Fr sh[QUO_TPB];
     const uint32_t t = threadIdx.x;
     Fr x;
-    sh[t] = quotient_xm1(gen, H, log_m, m, (uint64_t)blockIdx.x * QUO_TPB + t, x);
+    sh[t] = quotient_xm1(gen, H, log_m, ps, (uint64_t)blockIdx.x * QUO_TPB + t, x);
     __syncthreads();
     for (uint32_t s = QUO_TPB >> 1; s >= 1; s >>= 1) {
         if (t < s) sh[t] = sh[t] * sh[t + s];
@@ -123,7 +135,7 @@ __global__ void __launch_bounds__(QUO_TPB) quotient_inv_table_kernel(Fr gen, con
     __shared__ Fr tree[2 * QUO_TPB];
     const uint64_t i = (uint64_t)blockIdx.x * QUO_TPB + threadIdx.x;
     Fr x;
-    const Fr xm1 = quotient_xm1(gen, H, log_m, m, i, x);
+    const Fr xm1 = quotient_xm1(gen, H, log_m, QuotPts{m, 0, 1}, i, x);
     const Fr inv = block_batch_invert<QUO_TPB>(xm1, tree, prod_inv + blockIdx.x);
     if (i < m) gmem_st(table + i, inv);
 }
@@ -131,16 +143,17 @@ __global__ void __launch_bounds__(QUO_TPB) quotient_inv_table_kernel(Fr gen, con
 template <bool TABLE>
 __global__ void __launch_bounds__(QUO_TPB) quotient_kernel(QuotientArgs q) {
     const uint64_t i = (uint64_t)blockIdx.x * QUO_TPB + threadIdx.x;
-    const bool live = i < q.m;
+    const bool live = i < q.pts;
+    const uint64_t pt = q.first + (uint64_t)q.step * i;  // the point's index in the quotient coset
     const Fr one = Fr::one();
     Fr x, inv_xm1;
     if (TABLE) {
         if (!live) return;
-        x = q.gen * tw_lookup(q.H, i, q.log_m, 0);
-        inv_xm1 = gmem_ld(q.inv_xm1 + i);
+        x = q.gen * tw_lookup(q.H, pt, q.log_m, 0);
+        inv_xm1 = gmem_ld(q.inv_xm1 + pt);
     } else {
         __shared__ Fr tree[2 * QUO_TPB];
-        const Fr xm1 = quotient_xm1(q.gen, q.H, q.log_m, q.m, i, x);
+        const Fr xm1 = quotient_xm1(q.gen, q.H, q.log_m, QuotPts{q.pts, q.first, q.step}, i, x);
         inv_xm1 = block_batch_invert<QUO_TPB>(xm1, tree, q.prod_inv ? q.prod_inv + blockIdx.x : nullptr);
         if (!live) return;
     }
@@ -160,17 +173,17 @@ __global__ void __launch_bounds__(QUO_TPB) quotient_kernel(QuotientArgs q) {
     gate = gate - qmul(gmem_ld(q.sel[10] + i), e);
     // permutation constraint (lines 473-491): z(X) prod(w + beta k X + gamma) - z(omega X) prod(w + beta sigma + gamma)
     const Fr zi = gmem_ld(q.z + i);
-    Fr acc1 = zi, acc2 = gmem_ld(q.z + ((i + q.ratio) & (q.m - 1)));
+    Fr acc1 = zi, acc2 = gmem_ld(q.z + ((i + q.z_next) & (q.pts - 1)));
 #pragma unroll
     for (int j = 0; j < 5; j++) {
         const Fr t = wv[j] + q.gamma;
         acc1 = qmul(acc1, t + qmul(q.k_beta[j], x));
         acc2 = qmul(acc2, t + qmul(gmem_ld(q.sig[j] + i), q.beta));
     }
-    Fr r = qmul(q.zh_inv[i % q.ratio], gate + qmul(q.alpha, acc1 - acc2));
+    Fr r = qmul(q.zh_inv[pt % q.ratio], gate + qmul(q.alpha, acc1 - acc2));
     // (z - 1) L_1 alpha^2 / Z_H = alpha^2/n (z - 1) / (x - 1)   (lines 493-499)
     r = r + qmul(qmul(q.alpha_sq_div_n, zi - one), inv_xm1);
-    gmem_st(q.out + i, r);
+    gmem_st(q.out + pt, r);
 }
 
 // ------------------------------------------------------------------ p(z) and the suffix Horner scan

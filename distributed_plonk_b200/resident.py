@@ -27,13 +27,26 @@ from __future__ import annotations
 import numpy as np
 
 N_SEL, N_WIRE = 13, 5
+N_COEF = N_SEL + 2 * N_WIRE + 2       # polynomials evaluated on the quotient coset in round 3
 
 
 class ResidentProver:
-    def __init__(self, ctx, torch, log_n: int, device: str, field):
+    # Round 3 evaluates 25 polynomials of n coefficients on the m = 8n-point quotient coset.  "whole": 25 buffers of m points
+    # (25 x 8n x 32 B: 25 GiB at 2^22), one coset-NTT(8n) each, one quotient launch.  "sliced": the coset is the disjoint union
+    # of the 8 gate-domain cosets s_k * H_n (s_k = g * omega_m^k), so round 3 runs slice by slice through 25 n-point buffers:
+    # 25 slice transforms (dp_ntt_dev_quot_slice), then the quotient of that slice (dp_quotient_evals_slice_dev), which
+    # writes quot[k + 8i].  Same quotient bytes either way.  "auto" takes "whole" when its buffers fit the device's free memory
+    # with WHOLE_MARGIN_M quotient-domain buffers (the final iNTT(8n)'s scratch) and WHOLE_MARGIN_BYTES to spare, "sliced"
+    # otherwise.  (The cached 1/(x - 1) table of m points is optional: the quotient falls back to its tree variant without it.)
+    WHOLE_MARGIN_M, WHOLE_MARGIN_BYTES = 1, 1 << 30
+
+    def __init__(self, ctx, torch, log_n: int, device: str, field, quotient: str = "auto"):
         """field: helpers over raw Montgomery Fr as np.uint64[4] - mul(a,b), add(a,b), sub(a,b), inv(a), from_u64(v),
         pow_u64(a, e), omega (the generator of the n-point domain); tests and the bench pass the oracle's / numpy ones:
-        the handful of scalar challenge products of rounds 4-5 are host-side glue, not hot-path work"""
+        the handful of scalar challenge products of rounds 4-5 are host-side glue, not hot-path work.
+        quotient: "auto" (default), "whole" or "sliced" - how round 3 lays out its evaluations (above)"""
+        if quotient not in ("auto", "whole", "sliced"):
+            raise ValueError(f"quotient must be 'auto', 'whole' or 'sliced', not {quotient!r}")
         self.ctx, self.torch, self.F = ctx, torch, field
         self.log_n, self.n, self.m = log_n, 1 << log_n, 8 << log_n
         self.dev = device
@@ -50,11 +63,25 @@ class ResidentProver:
         self.pub = buf(n)
         self.wire_coef = [buf(n) for _ in range(N_WIRE)]
         self.z = buf(n)
-        self.big = [buf(m) for _ in range(N_SEL + 2 * N_WIRE + 2)]   # coset evaluations: 13 sel, 5 sigma, 5 wires, z, pub
         self.quot = buf(m)
         self.lin = buf(n + 2)
         self.batch = buf(n + 2)
         self.wit = [buf(n + 2), buf(n + 2)]
+        if quotient == "auto":
+            quotient = "whole" if self.whole_fits(torch, device, m) else "sliced"
+        self.quotient = quotient
+        # coset evaluations: 13 sel, 5 sigma, 5 wires, z, pub.  A whole-domain prover can also run the sliced round 3 (its
+        # slice buffers are the heads of the whole-domain ones): tools/bench_resident.py times both modes on one prover that way.
+        self.big = [buf(m) for _ in range(N_COEF)] if quotient == "whole" else None
+        self.slices = [t[:n] for t in self.big] if self.big is not None else [buf(n) for _ in range(N_COEF)]
+
+    @classmethod
+    def whole_fits(cls, torch, device: str, m: int) -> bool:
+        """the whole-domain layout fits the device's free memory with the stated margin (always on the CPU emulator)"""
+        if device == "cpu":
+            return True
+        free, _ = torch.cuda.mem_get_info(torch.device(device))
+        return (N_COEF + cls.WHOLE_MARGIN_M) * m * 32 + cls.WHOLE_MARGIN_BYTES <= free
 
     # ---- setup: the proving key, once
     def load_key(self, sel_coef, sig_coef, sig_eval, id_eval, k):
@@ -93,15 +120,23 @@ class ResidentProver:
         ctx.ntt_dev(P(self.z), log_n, True, False)
         com.append(ctx.commit_dev(P(self.z), n))
         ctx.ntt_dev(P(self.pub), log_n, True, False)
-        # round 3: 25 coset evaluations on the 8n domain; only the n coefficients at the head of each buffer are read
+        # round 3: 25 coset evaluations on the 8n domain, the quotient evaluations, one coset-iNTT(8n)
         srcs = self.sel_coef + self.sig_coef + self.wire_coef + [self.z, self.pub]
-        for dst, src in zip(self.big, srcs):
-            dst[:n].copy_(src)
-        self._sync()
-        for dst in self.big:
-            ctx.ntt_dev_padded(P(dst), n, log_m, False, True, wait=False)
-        b = [P(t) for t in self.big]
-        ctx.quotient_evals_dev(b[:13], b[13:18], b[18:23], b[23], b[24], self.k, ch["alpha"], ch["beta"], ch["gamma"], P(self.quot))
+        qargs = (self.k, ch["alpha"], ch["beta"], ch["gamma"])
+        if self.quotient == "whole":   # only the n coefficients at the head of each buffer are read
+            for dst, src in zip(self.big, srcs):
+                dst[:n].copy_(src)
+            self._sync()
+            for dst in self.big:
+                ctx.ntt_dev_padded(P(dst), n, log_m, False, True, wait=False)
+            b = [P(t) for t in self.big]
+            ctx.quotient_evals_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, P(self.quot))
+        else:                          # slice k into the same 25 n-point buffers, every k; all of it on the library's stream
+            b = [P(t) for t in self.slices]
+            for k in range(m // n):
+                for dst, src in zip(b, srcs):
+                    ctx.ntt_dev_quot_slice(P(src), n, k, dst, wait=False)
+                ctx.quotient_evals_slice_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, k, P(self.quot))
         ctx.ntt_dev(P(self.quot), log_m, True, True)
         chunk = n + 2
         for j in range(N_WIRE):
@@ -188,15 +223,16 @@ class NumpyField:
         return self._enc(pow(self._dec(a), e, self.R_MOD))
 
 
-def bench_leg(ctx, torch, log_n: int, rand_fr, timed, steps: int = 3):
-    """bench.py's e2e_resident: proofs/s of ResidentProver.prove on synthetic data (random polynomials: the
-    arithmetic is data-independent; the quotient is then not a polynomial of the expected degree, which changes
-    nothing about the work), witness copied from pinned host memory inside the timed region"""
-    if log_n > 22:
-        return {"skipped": f"2^{log_n}: 25 resident coset evaluations need {25 * (8 << log_n) * 32 / 2**30:.0f} GiB"}
+def _gib(b) -> float:
+    return round(b / 2**30, 3)
+
+
+def make_bench_prover(ctx, torch, log_n: int, rand_fr, quotient: str = "auto"):
+    """a ResidentProver on synthetic data (random polynomials: the arithmetic is data-independent; the quotient is then not
+    a polynomial of the expected degree, which changes nothing about the work), with the witness in pinned host memory"""
     n = 1 << log_n
     F = NumpyField(log_n)
-    pr = ResidentProver(ctx, torch, log_n, "cuda", F)
+    pr = ResidentProver(ctx, torch, log_n, "cuda", F, quotient=quotient)
     for t in pr.sel_coef + pr.sig_coef:
         t.copy_(rand_fr(n))
     pr.sig_eval.copy_(rand_fr(N_WIRE * n))
@@ -205,6 +241,22 @@ def bench_leg(ctx, torch, log_n: int, rand_fr, timed, steps: int = 3):
     wires = rand_fr(N_WIRE * n).cpu().pin_memory()
     pub = rand_fr(n).cpu().pin_memory()
     ch = {name: F.from_u64(v) for name, v in (("beta", 0xB17A), ("gamma", 0x6A33A), ("alpha", 0xA1FA), ("zeta", 0x2E7A), ("v", 0x55))}
+    return pr, (wires, pub, ch)
+
+
+def bench_leg(ctx, torch, log_n: int, rand_fr, timed, steps: int = 3, quotient: str = "auto", prover=None):
+    """bench.py's e2e_resident: proofs/s of ResidentProver.prove on synthetic data, witness copied from pinned host memory
+    inside the timed region.  The prover picks its round-3 layout (quotient="auto") unless told; `prover` = (pr, inputs) of
+    make_bench_prover to time an existing one (tools/bench_resident.py).  Also records the layout and the leg's peak device
+    memory: torch's peak plus what the library's pool added (cudaMemGetInfo before and after; the pool keeps what it
+    allocates).  Torch's cached free blocks are returned to the device first, so that the layout is chosen on what is free."""
+    if prover is None:
+        torch.cuda.empty_cache()
+    free0, total = torch.cuda.mem_get_info()
+    res0 = torch.cuda.memory_reserved()
+    torch.cuda.reset_peak_memory_stats()
+    pr, (wires, pub, ch) = prover if prover is not None else make_bench_prover(ctx, torch, log_n, rand_fr, quotient)
+    n = 1 << log_n
     out = {}
 
     def step():
@@ -212,9 +264,18 @@ def bench_leg(ctx, torch, log_n: int, rand_fr, timed, steps: int = 3):
 
     dt, _ = timed(step, steps, 1, False)
     com, ev = out["r"]
-    return {"value": steps / dt, "unit": "proofs/s", "ms_per_step": dt / steps * 1e3, "steps": steps,
-            "h2d_bytes_per_step": int((N_WIRE + 1) * n * 32), "d2h_bytes_per_step": int(len(com) * 144 + len(ev) * 32),
+    free1, _ = torch.cuda.mem_get_info()
+    res1, torch_peak = torch.cuda.memory_reserved(), torch.cuda.max_memory_reserved()
+    lib_added = max(0, (free0 - free1) - (res1 - res0))
+    in_use_before = total - free0
+    mem = {"peak_gib": _gib(in_use_before - res0 + torch_peak + lib_added), "torch_peak_reserved_gib": _gib(torch_peak),
+           "library_added_gib": _gib(lib_added), "in_use_before_gib": _gib(in_use_before), "device_total_gib": _gib(total),
+           "how": "device memory in use before the leg, minus torch's reserve then, plus torch's peak reserve during the leg, plus "
+                  "what the library's pool grew by (its blocks are cached, so its end size is its peak)"}
+    return {"value": steps / dt, "unit": "proofs/s", "ms_per_step": dt / steps * 1e3, "steps": steps, "quotient": pr.quotient,
+            "device_memory": mem, "h2d_bytes_per_step": int((N_WIRE + 1) * n * 32), "d2h_bytes_per_step": int(len(com) * 144 + len(ev) * 32),
             "what": ("rounds 1-5 of one proof on worker-resident polynomials (distributed_plonk_b200/resident.py): witness in once, "
                      "13 commitments + 10 evaluations out; includes the round-2 grand product, the quotient evaluations, the round-4 "
-                     "evaluations and the round-5 folds / divisions that the 33-transform + 13-MSM schedule of `value` leaves to the dispatcher"),
+                     "evaluations and the round-5 folds / divisions that the 33-transform + 13-MSM schedule of `value` leaves to the dispatcher; "
+                     "quotient = round 3's layout: whole (25 buffers of 8n points) or sliced (8 slices through 25 buffers of n points)"),
             "timing": "host clock between barrier+synchronize"}

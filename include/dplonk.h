@@ -210,6 +210,19 @@ typedef struct dp_quotient_args {
 int dp_quotient_evals(dp_ctx *ctx, const dp_quotient_args *host_arrays, void *out);
 int dp_quotient_evals_dev(dp_ctx *ctx, const dp_quotient_args *dev_arrays, void *out_dev);
 
+/* Round 3 one slice at a time, with n-sized instead of m-sized evaluation buffers (n, m = the two domains given to
+ * dp_init, m/n slices).  The quotient coset is the disjoint union of m/n cosets of the gate domain:
+ * g * omega_m^(slice + (m/n) i) = s * omega_n^i, s = g * omega_m^slice, i < n.
+ * p(s * omega_n^i), i < n: slice `slice` of the coset evaluation on the quotient domain.  coeffs_dev: n_valid <= n
+ * coefficients, not modified (entries past n_valid are not read); out_dev: n Fr, must not overlap coeffs_dev.
+ * wait = 0 returns once queued (dp_sync waits).  DP_E_STATE before dp_init; DP_E_ARG for slice >= m/n, n_valid > n,
+ * NULL pointers or overlapping buffers.                                                                            */
+int dp_ntt_dev_quot_slice(dp_ctx *ctx, const void *coeffs_dev, size_t n_valid, uint32_t slice, void *out_dev, int wait);
+/* dp_quotient_evals_dev for one slice: the 25 arrays hold n Fr each (slice `slice` of the coset evaluations, as
+ * dp_ntt_dev_quot_slice writes them); writes out_dev[slice + (m/n) i], i < n, of the m-entry output and nothing else.
+ * All m/n slices = dp_quotient_evals_dev, byte for byte.  Same errors as dp_ntt_dev_quot_slice.                    */
+int dp_quotient_evals_slice_dev(dp_ctx *ctx, const dp_quotient_args *slice_arrays, uint32_t slice, void *out_dev);
+
 /* Round 4, DensePolynomial::evaluate (src/dispatcher2.rs:535-548): out32 = sum_j coeffs[j] * point^j */
 int dp_poly_eval(dp_ctx *ctx, const void *coeffs, size_t n, const void *point, void *out32);
 int dp_poly_eval_dev(dp_ctx *ctx, const void *coeffs_dev, size_t n, const void *point, void *out32);

@@ -21,6 +21,20 @@ pub struct dp_fft_workload {
 
 pub const DP_IPC_HANDLE_BYTES: usize = 64;
 
+/// the 25 coset-evaluation arrays and the challenges of round 3 (include/dplonk.h: dp_quotient_args)
+#[repr(C)]
+pub struct dp_quotient_args {
+    pub selectors: [*const c_void; 13],
+    pub sigmas: [*const c_void; 5],
+    pub wires: [*const c_void; 5],
+    pub perm: *const c_void,
+    pub pub_input: *const c_void,
+    pub k: *const u8,
+    pub alpha: *const u8,
+    pub beta: *const u8,
+    pub gamma: *const u8,
+}
+
 extern "C" {
     pub fn dp_create(cuda_device: c_int, me: u64, n_workers: u64, out: *mut *mut dp_ctx) -> c_int;
     pub fn dp_destroy(ctx: *mut dp_ctx) -> c_int;
@@ -45,6 +59,11 @@ extern "C" {
     pub fn dp_fft2(ctx: *mut dp_ctx, id: u64, out: *mut u8, out_bytes: usize) -> c_int;
     pub fn dp_round1(ctx: *mut dp_ctx, evals: *const u8, n: usize, blind_2fr: *const u8, out144: *mut u8) -> c_int;
     pub fn dp_get_wire(ctx: *mut dp_ctx, out: *mut u8, out_bytes: usize, n_coeffs: *mut usize) -> c_int;
+    pub fn dp_quotient_evals_dev(ctx: *mut dp_ctx, dev_arrays: *const dp_quotient_args, out_dev: *mut c_void) -> c_int;
+    pub fn dp_ntt_dev_quot_slice(ctx: *mut dp_ctx, coeffs_dev: *const c_void, n_valid: usize, slice: u32, out_dev: *mut c_void,
+                                 wait: c_int) -> c_int;
+    pub fn dp_quotient_evals_slice_dev(ctx: *mut dp_ctx, slice_arrays: *const dp_quotient_args, slice: u32,
+                                       out_dev: *mut c_void) -> c_int;
     pub fn dp_peer_arena_create(ctx: *mut dp_ctx, arena_bytes: u64, handle_out: *mut u8) -> c_int;
     pub fn dp_peer_attach(ctx: *mut dp_ctx, peer: u64, handle: *const u8) -> c_int;
     pub fn dp_peer_ready(ctx: *const dp_ctx) -> c_int;
