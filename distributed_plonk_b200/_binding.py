@@ -19,6 +19,7 @@ EXPORTS = [
     "dp_msm_submit", "dp_msm_collect", "dp_poly_put", "dp_poly_ptr", "dp_poly_get", "dp_poly_free", "dp_commit_dev",
     "dp_fft_exchange_begin_async", "dp_compute_stream", "dp_fft_dev_p2p_async", "dp_fft1_rows_short", "dp_fft_dev_hint_valid_cols", "dp_ntt_dev_padded", "dp_debug_set_three_pass",
     "dp_ntt_dev_quot_slice", "dp_quotient_evals_slice_dev",
+    "dp_poly_blind_dev", "dp_quotient_evals_tail_dev", "dp_quotient_evals_slice_tail_dev",
 ]
 
 
@@ -37,6 +38,11 @@ class QuotientArgs(C.Structure):
     """dp_quotient_args (include/dplonk.h): 25 polynomial-sized arrays + the challenges"""
     _fields_ = [("selectors", C.c_void_p * 13), ("sigmas", C.c_void_p * 5), ("wires", C.c_void_p * 5), ("perm", C.c_void_p),
                 ("pub_input", C.c_void_p), ("k", C.c_void_p), ("alpha", C.c_void_p), ("beta", C.c_void_p), ("gamma", C.c_void_p)]
+
+
+class QuotientTails(C.Structure):
+    """dp_quotient_tails (include/dplonk.h): coefficients n, n+1, ... of each blinded wire and of z (device pointers)"""
+    _fields_ = [("wires", C.c_void_p * 5), ("wire_len", C.c_size_t * 5), ("perm", C.c_void_p), ("perm_len", C.c_size_t)]
 
 
 def bind(cdll: C.CDLL) -> C.CDLL:
@@ -101,6 +107,9 @@ def bind(cdll: C.CDLL) -> C.CDLL:
         "dp_quotient_evals_dev": (i, [vp, C.POINTER(QuotientArgs), vp]),
         "dp_quotient_evals_slice_dev": (i, [vp, C.POINTER(QuotientArgs), u32, vp]),
         "dp_ntt_dev_quot_slice": (i, [vp, vp, sz, u32, vp, i]),
+        "dp_quotient_evals_tail_dev": (i, [vp, C.POINTER(QuotientArgs), C.POINTER(QuotientTails), vp]),
+        "dp_quotient_evals_slice_tail_dev": (i, [vp, C.POINTER(QuotientArgs), C.POINTER(QuotientTails), u32, vp]),
+        "dp_poly_blind_dev": (i, [vp, vp, sz, u32, vp]),
         "dp_poly_eval": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_eval_dev": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_lincomb": (i, [vp, C.POINTER(vp), C.POINTER(sz), vp, sz, vp, sz]),
@@ -336,6 +345,37 @@ class Context:
         keep = []
         q = self._quotient_args(selectors, sigmas, wires, perm, pub_input, k, alpha, beta, gamma, keep)
         self._ck(self.lib.dp_quotient_evals_slice_dev(self.h, C.byref(q), slice_, out_ptr))
+
+    @staticmethod
+    def _quotient_tails(tails) -> QuotientTails:
+        """tails: 6 (device pointer or None, length) pairs, the five wires then z"""
+        t = QuotientTails()
+        for j, (ptr, ln) in enumerate(tails[:5]):
+            t.wires[j], t.wire_len[j] = ptr, ln
+        t.perm, t.perm_len = tails[5]
+        return t
+
+    def quotient_evals_tail_dev(self, selectors, sigmas, wires, perm, pub_input, k, alpha, beta, gamma, tails, out_ptr: int):
+        """quotient_evals_dev of blinded wires and z: the arrays hold the evaluations of their first n coefficients, `tails`
+        gives coefficients n, n+1, ... of each (6 (pointer, length) pairs, wires then z, lengths <= 3)"""
+        keep = []
+        q = self._quotient_args(selectors, sigmas, wires, perm, pub_input, k, alpha, beta, gamma, keep)
+        t = self._quotient_tails(tails)
+        self._ck(self.lib.dp_quotient_evals_tail_dev(self.h, C.byref(q), C.byref(t), out_ptr))
+
+    def quotient_evals_slice_tail_dev(self, selectors, sigmas, wires, perm, pub_input, k, alpha, beta, gamma, tails, slice_: int,
+                                      out_ptr: int):
+        """quotient_evals_slice_dev of blinded wires and z (quotient_evals_tail_dev)"""
+        keep = []
+        q = self._quotient_args(selectors, sigmas, wires, perm, pub_input, k, alpha, beta, gamma, keep)
+        t = self._quotient_tails(tails)
+        self._ck(self.lib.dp_quotient_evals_slice_tail_dev(self.h, C.byref(q), C.byref(t), slice_, out_ptr))
+
+    def poly_blind_dev(self, coeffs_ptr: int, n: int, k: int, blind: np.ndarray | None = None):
+        """coeffs += b(X) * (X^n - 1) in place (n + k Fr on the device); blind = [k,4] raw Fr, or None: the library draws
+        the k scalars from the OS entropy pool and they never leave it"""
+        b = np.ascontiguousarray(blind, dtype=np.uint64) if blind is not None else None
+        self._ck(self.lib.dp_poly_blind_dev(self.h, coeffs_ptr, n, k, _addr(b) if b is not None else None))
 
     def poly_eval(self, coeffs, point: np.ndarray, n: int | None = None) -> np.ndarray:
         """round 4: p(point); coeffs = [n,4] host array, or a device pointer with n given"""

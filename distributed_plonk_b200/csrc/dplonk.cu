@@ -2227,19 +2227,38 @@ int dp_ntt(dp_ctx *ctx, void *data, size_t n, uint32_t log_n, int is_inv, int is
     return call_end(ctx, true);
 }
 
-// wire = (b0 + b1*X) * (X^n - 1) + poly   (worker.rs:400-401)
-__global__ void round1_blind_kernel(Fr *wire, uint64_t n, Fr b0, Fr b1) {
+// coeffs += b(X) * (X^n - 1), b = b_0 + b_1 X + ... + b_(k-1) X^(k-1), k <= RND_MAX_TAIL: for each j in turn, b_j comes
+// off coefficient j and onto coefficient n + j.  For n < k the two ranges meet, and the order gives the right sum: n == 1,
+// k == 2 leaves c_1 + b_0 - b_1 at index 1 (worker.rs:400-401 blinds a wire with k = 2)
+struct BlindScalars {
+    Fr b[RND_MAX_TAIL];
+};
+__global__ void poly_blind_kernel(Fr *coeffs, uint64_t n, uint32_t k, BlindScalars s) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
-    if (n >= 2) {
-        wire[0] = wire[0] - b0;
-        wire[1] = wire[1] - b1;
-        wire[n] = b0;
-        wire[n + 1] = b1;
-    } else {  // n == 1: X^1 - 1
-        wire[0] = wire[0] - b0;
-        wire[1] = b0 - b1;
-        wire[2] = b1;
+    for (uint32_t j = 0; j < k; j++) {
+        coeffs[j] = coeffs[j] - s.b[j];
+        coeffs[n + j] = coeffs[n + j] + s.b[j];
     }
+}
+
+// k secret scalars, uniform over [0, r).  The reference blinds with ThreadRng, a CSPRNG (worker.rs:400, dispatcher2.rs:
+// 294-361): the scalars must be unpredictable, so they come from the kernel's entropy pool, as canonical residues < r by
+// rejection (r is 255 bits: one try in ~2.2 is rejected).  Any residue < r is a valid Montgomery-form element.
+static int draw_secret_fr(dp_ctx *ctx, Fr *out, uint32_t k, const char *who) {
+    for (uint32_t j = 0; j < k; j++) {
+        Fr v;
+        do {
+            size_t got = 0;
+            while (got < sizeof(Fr)) {
+                const ssize_t r = getrandom(reinterpret_cast<uint8_t *>(v.l) + got, sizeof(Fr) - got, 0);
+                if (r < 0) return fail(ctx, DP_E_STATE, "%s: getrandom failed; pass the blinders in `blind`", who);
+                got += (size_t)r;
+            }
+            v.l[7] &= 0x7fffffffu;
+        } while (!v.canon_is_reduced());
+        out[j] = v;
+    }
+    return DP_OK;
 }
 
 int dp_round1(dp_ctx *ctx, const void *evals, size_t n, const void *blind, void *out) {
@@ -2260,32 +2279,37 @@ int dp_round1(dp_ctx *ctx, const void *evals, size_t n, const void *blind, void 
     DP_CUDA(ctx, cudaMemcpyAsync(ctx->wire, evals, n * sizeof(Fr), cudaMemcpyHostToDevice, ctx->stream));
     DP_CUDA(ctx, cudaMemsetAsync(ctx->wire + n, 0, (N + 2 - n) * sizeof(Fr), ctx->stream));
     DP_TRY(ntt_device(ctx, ctx->wire, d.log_n, true, false));
-    Fr b[2];
-    if (blind) {
-        memcpy(b, blind, sizeof b);
-    } else {
-        // The reference blinds with ThreadRng, a CSPRNG (worker.rs:400): the two scalars must be unpredictable,
-        // so they come from the kernel's entropy pool: uniform canonical residues < r by rejection (r is 255
-        // bits: one try in ~2.2 is rejected).  Any residue < r is a valid Montgomery-form element.
-        for (int k = 0; k < 2; k++) {
-            Fr v;
-            do {
-                size_t got = 0;
-                while (got < sizeof(Fr)) {
-                    const ssize_t r = getrandom(reinterpret_cast<uint8_t *>(v.l) + got, sizeof(Fr) - got, 0);
-                    if (r < 0) return fail(ctx, DP_E_STATE, "dp_round1: getrandom failed; pass the blinders in `blind`");
-                    got += (size_t)r;
-                }
-                v.l[7] &= 0x7fffffffu;
-            } while (!v.canon_is_reduced());
-            b[k] = v;
-        }
-    }
-    DP_LAUNCH(round1_blind_kernel, dim3(1), dim3(32), 0, ctx->stream, ctx->wire, N, b[0], b[1]);
+    BlindScalars b;
+    memset((void *)&b, 0, sizeof b);
+    if (blind) memcpy(b.b, blind, 2 * sizeof(Fr));
+    else DP_TRY(draw_secret_fr(ctx, b.b, 2, "dp_round1"));
+    DP_LAUNCH(poly_blind_kernel, dim3(1), dim3(32), 0, ctx->stream, ctx->wire, N, 2u, b);
     ctx->launches++;
     DP_TRY(commit_device(ctx, ctx->wire, N + 2, od));
     DP_CUDA(ctx, cudaMemcpyAsync(out, od, sizeof(G1JacobianOut), cudaMemcpyDeviceToHost, ctx->stream));
     return call_end(ctx, true);
+}
+
+int dp_poly_blind_dev(dp_ctx *ctx, void *coeffs_dev, size_t n, uint32_t k, const void *blind) {
+    if (!ctx || !coeffs_dev) return fail(ctx, DP_E_ARG, "dp_poly_blind_dev: NULL argument");
+    if (k > RND_MAX_TAIL) return fail(ctx, DP_E_ARG, "dp_poly_blind_dev: %u blinding scalars, at most %u", k, RND_MAX_TAIL);
+    BlindScalars b;
+    memset((void *)&b, 0, sizeof b);
+    if (blind) {
+        memcpy(b.b, blind, k * sizeof(Fr));
+        for (uint32_t j = 0; j < k; j++)
+            if (!b.b[j].canon_is_reduced()) return fail(ctx, DP_E_ARG, "dp_poly_blind_dev: blinding scalar %u is not below r", j);
+    } else {
+        DP_TRY(draw_secret_fr(ctx, b.b, k, "dp_poly_blind_dev"));
+    }
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    DP_LAUNCH(poly_blind_kernel, dim3(1), dim3(32), 0, ctx->stream, (Fr *)coeffs_dev, (uint64_t)n, k, b);
+    ctx->launches++;
+    DP_CUDA(ctx, cudaGetLastError());
+    const int rc = call_end(ctx, true);
+    explicit_bzero((void *)&b, sizeof b);   // drawn scalars never leave the library; the launch copied its parameters
+    return rc;
 }
 
 // multiplicative scan of n Fr on the compute stream: out[i] = product of the logical elements before
@@ -2609,8 +2633,10 @@ int poly_suffix_device(dp_ctx *ctx, const Fr *in, uint64_t n, const Fr *pw, uint
 
 // slice < 0: the whole quotient coset (25 arrays of m points); else slice k of it (25 arrays of n points, DESIGN.md 3.4):
 // points g * omega_m^(k + (m/n) i), written to out_dev[k + (m/n) i]
+// tails (checked by quotient_tails_check, not all empty): the wires and z have more than n coefficients, the arrays hold the
+// evaluations of their first n (QuotientTailArgs)
 int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arrays /* 25 device arrays */, Fr *out_dev,
-                    int slice = -1) {
+                    int slice = -1, const dp_quotient_tails *tails = nullptr) {
     const DomainDev &dq = ctx->dom[1], &dg = ctx->dom[0];
     const uint64_t m = dq.n(), n = dg.n();
     if (m < n || m / n > RND_MAX_RATIO) return fail(ctx, DP_E_ARG, "quotient domain / gate domain = %llu, supported: 1..%d", (unsigned long long)(m / n), RND_MAX_RATIO);
@@ -2631,11 +2657,12 @@ int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arr
     q.ratio = (uint32_t)(m / n);
     // 1 / Z_H(x_i), x_i = g omega_m^i, i < m/n: x_i^n = g^n (omega_m^n)^i   (dispatcher2.rs:372-379)
     const Fr gn = q.gen.pow(n), wn = fr_domain_gen(dq.log_n).pow(n);
-    Fr cur = gn;
+    Fr cur = gn, xn[RND_MAX_RATIO];
     for (uint32_t i = 0; i < q.ratio; i++) {
         const Fr zh = cur - Fr::one();
         if (zh.is_zero()) return fail(ctx, DP_E_ARG, "Z_H vanishes on the quotient coset (domains %llu / %llu)", (unsigned long long)n, (unsigned long long)m);
         q.zh_inv[i] = zh.inverse();
+        xn[i] = cur;
         cur = cur * wn;
     }
     for (uint32_t i = q.ratio; i < RND_MAX_RATIO; i++) q.zh_inv[i] = Fr::zero();
@@ -2677,21 +2704,39 @@ int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arr
     }
     q.prod_inv = nullptr;
     q.inv_xm1 = nullptr;
-    if (want_table && ctx->quot_inv) {
-        q.inv_xm1 = ctx->quot_inv;
-        DP_LAUNCH(quotient_kernel<true>, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, q);
-        ctx->launches += 1;
-    } else {
-        Fr *prod = tmp.get<Fr>(n_blocks);
-        if (!prod) return fail(ctx, DP_E_OOM, "quotient scratch");
-        DP_LAUNCH(quotient_xm1_products_kernel, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, q.gen, q.H, q.log_m, pts, prod);
-        DP_LAUNCH(fr_invert_kernel, dim3(blocks_for(n_blocks, 128)), dim3(128), 0, ctx->stream, prod, (uint64_t)n_blocks);
-        q.prod_inv = prod;
-        DP_LAUNCH(quotient_kernel<false>, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, q);
-        ctx->launches += 3;
+    // the same launches with either argument type: QuotientArgs, or QuotientTailArgs for blinded wires and z
+    auto launch = [&](auto &args) -> int {
+        using Args = std::decay_t<decltype(args)>;
+        if (want_table && ctx->quot_inv) {
+            args.inv_xm1 = ctx->quot_inv;
+            const auto kernel = quotient_kernel<true, Args>;
+            DP_LAUNCH(kernel, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, args);
+            ctx->launches += 1;
+        } else {
+            Fr *prod = tmp.get<Fr>(n_blocks);
+            if (!prod) return fail(ctx, DP_E_OOM, "quotient scratch");
+            DP_LAUNCH(quotient_xm1_products_kernel, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, q.gen, q.H, q.log_m, pts, prod);
+            DP_LAUNCH(fr_invert_kernel, dim3(blocks_for(n_blocks, 128)), dim3(128), 0, ctx->stream, prod, (uint64_t)n_blocks);
+            args.prod_inv = prod;
+            const auto kernel = quotient_kernel<false, Args>;
+            DP_LAUNCH(kernel, dim3(n_blocks), dim3(QUO_TPB), 0, ctx->stream, args);
+            ctx->launches += 3;
+        }
+        DP_CUDA(ctx, cudaGetLastError());
+        return DP_OK;
+    };
+    if (!tails) return launch(q);
+    QuotientTailArgs qt;
+    static_cast<QuotientArgs &>(qt) = q;
+    for (int j = 0; j < 5; j++) {
+        qt.w_tail[j] = (const Fr *)tails->wires[j];
+        qt.w_tail_len[j] = (uint32_t)tails->wire_len[j];
     }
-    DP_CUDA(ctx, cudaGetLastError());
-    return DP_OK;
+    qt.z_tail = (const Fr *)tails->perm;
+    qt.z_tail_len = (uint32_t)tails->perm_len;
+    for (uint32_t i = 0; i < RND_MAX_RATIO; i++) qt.xn[i] = i < q.ratio ? xn[i] : Fr::zero();
+    qt.omega_n = fr_domain_gen(dg.log_n);
+    return launch(qt);
 }
 
 const void *const *quotient_ptrs(const dp_quotient_args &a, const void *flat[25]) {
@@ -2701,6 +2746,24 @@ const void *const *quotient_ptrs(const dp_quotient_args &a, const void *flat[25]
     flat[23] = a.perm;
     flat[24] = a.pub_input;
     return flat;
+}
+
+// DP_E_ARG for a tail longer than RND_MAX_TAIL, a NULL tail of nonzero length, or one that overlaps the m-entry output.
+// *any = some tail is not empty.
+int quotient_tails_check(dp_ctx *ctx, const dp_quotient_tails *t, const void *out, bool *any, const char *who) {
+    if (!t) return fail(ctx, DP_E_ARG, "%s: NULL tails", who);
+    const uint64_t m = ctx->dom[1].n();
+    *any = false;
+    for (int j = 0; j < 6; j++) {
+        const void *p = j < 5 ? t->wires[j] : t->perm;
+        const size_t len = j < 5 ? t->wire_len[j] : t->perm_len;
+        if (len > RND_MAX_TAIL) return fail(ctx, DP_E_ARG, "%s: tail %d has %zu coefficients, at most %u", who, j, len, RND_MAX_TAIL);
+        if (!len) continue;
+        if (!p) return fail(ctx, DP_E_ARG, "%s: tail %d is NULL", who, j);
+        if (ranges_overlap(p, len * sizeof(Fr), out, m * sizeof(Fr))) return fail(ctx, DP_E_ARG, "%s: the output overlaps tail %d", who, j);
+        *any = true;
+    }
+    return DP_OK;
 }
 
 int quotient_check(dp_ctx *ctx, const dp_quotient_args *a, const void *out, const char *who) {
@@ -2750,20 +2813,45 @@ int dp_quotient_evals_dev(dp_ctx *ctx, const dp_quotient_args *a, void *out_dev)
     return call_end(ctx, true);
 }
 
-int dp_quotient_evals_slice_dev(dp_ctx *ctx, const dp_quotient_args *slice_arrays, uint32_t slice, void *out_dev) {
-    DP_TRY(quotient_check(ctx, slice_arrays, out_dev, "dp_quotient_evals_slice_dev"));
+int dp_quotient_evals_tail_dev(dp_ctx *ctx, const dp_quotient_args *a, const dp_quotient_tails *tails, void *out_dev) {
+    DP_TRY(quotient_check(ctx, a, out_dev, "dp_quotient_evals_tail_dev"));
+    bool any = false;
+    DP_TRY(quotient_tails_check(ctx, tails, out_dev, &any, "dp_quotient_evals_tail_dev"));
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    const void *flat[25];
+    quotient_ptrs(*a, flat);
+    DP_TRY(quotient_device(ctx, *a, reinterpret_cast<const Fr *const *>(flat), (Fr *)out_dev, -1, any ? tails : nullptr));
+    return call_end(ctx, true);
+}
+
+static int quotient_slice_any(dp_ctx *ctx, const dp_quotient_args *slice_arrays, const dp_quotient_tails *tails, uint32_t slice,
+                              void *out_dev, const char *who) {
+    DP_TRY(quotient_check(ctx, slice_arrays, out_dev, who));
+    bool any = false;
+    if (tails) DP_TRY(quotient_tails_check(ctx, tails, out_dev, &any, who));
     const DomainDev &dg = ctx->dom[0], &dq = ctx->dom[1];
     const uint64_t n = dg.n(), m = dq.n();
-    if (m < n || slice >= m / n) return fail(ctx, DP_E_ARG, "dp_quotient_evals_slice_dev: slice %u of %llu", slice, (unsigned long long)(m < n ? 0 : m / n));
+    if (m < n || slice >= m / n) return fail(ctx, DP_E_ARG, "%s: slice %u of %llu", who, slice, (unsigned long long)(m < n ? 0 : m / n));
     const void *flat[25];
     quotient_ptrs(*slice_arrays, flat);
     for (int i = 0; i < 25; i++)
         if (ranges_overlap(flat[i], n * sizeof(Fr), out_dev, m * sizeof(Fr)))
-            return fail(ctx, DP_E_ARG, "dp_quotient_evals_slice_dev: the output overlaps input %d", i);
+            return fail(ctx, DP_E_ARG, "%s: the output overlaps input %d", who, i);
     DP_CUDA(ctx, cudaSetDevice(ctx->device));
     call_begin(ctx);
-    DP_TRY(quotient_device(ctx, *slice_arrays, reinterpret_cast<const Fr *const *>(flat), (Fr *)out_dev, (int)slice));
+    DP_TRY(quotient_device(ctx, *slice_arrays, reinterpret_cast<const Fr *const *>(flat), (Fr *)out_dev, (int)slice, any ? tails : nullptr));
     return call_end(ctx, true);
+}
+
+int dp_quotient_evals_slice_dev(dp_ctx *ctx, const dp_quotient_args *slice_arrays, uint32_t slice, void *out_dev) {
+    return quotient_slice_any(ctx, slice_arrays, nullptr, slice, out_dev, "dp_quotient_evals_slice_dev");
+}
+
+int dp_quotient_evals_slice_tail_dev(dp_ctx *ctx, const dp_quotient_args *slice_arrays, const dp_quotient_tails *tails, uint32_t slice,
+                                     void *out_dev) {
+    if (!tails) return fail(ctx, DP_E_ARG, "dp_quotient_evals_slice_tail_dev: NULL tails");
+    return quotient_slice_any(ctx, slice_arrays, tails, slice, out_dev, "dp_quotient_evals_slice_tail_dev");
 }
 
 static int poly_eval_any(dp_ctx *ctx, const void *coeffs, size_t n, const void *point, void *out32, bool on_device, const char *who) {

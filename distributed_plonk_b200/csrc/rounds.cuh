@@ -7,7 +7,8 @@
 // polynomials resident on the worker these are four small families of kernels:
 //   * quotient_kernel        one thread per point of the quotient domain, or of one n-point slice of it
 //                            (DESIGN.md 3.4); the 1/(x_i - 1) of the L_1 term come from a cached table or
-//                            from ONE inversion per block (product tree in shared memory)
+//                            from ONE inversion per block (product tree in shared memory); the tail variant
+//                            adds the blinding coefficients of the wires and z as it loads them
 //   * poly_fold_kernel       p(z): Horner per thread, tree per block, recursion over block results
 //   * poly_suffix_kernel     E_j = sum_{k>=j} p_k z^(k-j): the quotient by (X - z) is E shifted by one,
 //                            E_0 is the remainder p(z); same chunking, carries from a recursive scan
@@ -15,6 +16,8 @@
 // Every result is a canonical Montgomery Fr, so equal values are equal bytes: parity with the
 // reference's sequential code is bit-exact by construction, whatever the order of operations.
 #pragma once
+#include <type_traits>
+
 #include "ntt.cuh"
 
 namespace dp {
@@ -140,8 +143,33 @@ __global__ void __launch_bounds__(QUO_TPB) quotient_inv_table_kernel(Fr gen, con
     if (i < m) gmem_st(table + i, inv);
 }
 
-template <bool TABLE>
-__global__ void __launch_bounds__(QUO_TPB) quotient_kernel(QuotientArgs q) {
+// Blinded inputs (DESIGN.md 3.4): a wire or z with n + t coefficients (t <= 3) is p = head + X^n tail.  The 25 arrays hold
+// the evaluations of the heads (n coefficients, the usual coset transforms); the kernel adds x^n tail(x) to each blinded
+// input as it loads it, and x^n tail(omega_n x) to z(omega x), since (omega_n x)^n = x^n.  x^n takes one value per slice
+// class pt mod ratio: the same constants whose inverses zh_inv holds shifted by one.
+constexpr uint32_t RND_MAX_TAIL = 3;
+struct QuotientTailArgs : QuotientArgs {
+    const Fr *w_tail[5];   // coefficients n, n+1, ... of each wire (device; read by every thread)
+    const Fr *z_tail;
+    uint32_t w_tail_len[5], z_tail_len;
+    Fr xn[RND_MAX_RATIO];  // x_i^n, i < ratio
+    Fr omega_n;
+};
+
+// t[0] + t[1] y + ... + t[len - 1] y^(len - 1), len <= RND_MAX_TAIL (uniform across the launch): len - 1 products
+DP_D Fr quotient_tail_at(const Fr *t, uint32_t len, const Fr &y) {
+    Fr acc = Fr::zero();
+#pragma unroll
+    for (int j = (int)RND_MAX_TAIL - 1; j >= 0; j--) {
+        if ((uint32_t)j + 1 < len) acc = qmul(acc, y) + gmem_ld(t + j);
+        else if ((uint32_t)j + 1 == len) acc = gmem_ld(t + j);
+    }
+    return acc;
+}
+
+template <bool TABLE, typename Args = QuotientArgs>
+__global__ void __launch_bounds__(QUO_TPB) quotient_kernel(Args q) {
+    constexpr bool TAIL = std::is_same<Args, QuotientTailArgs>::value;
     const uint64_t i = (uint64_t)blockIdx.x * QUO_TPB + threadIdx.x;
     const bool live = i < q.pts;
     const uint64_t pt = q.first + (uint64_t)q.step * i;  // the point's index in the quotient coset
@@ -157,7 +185,14 @@ __global__ void __launch_bounds__(QUO_TPB) quotient_kernel(QuotientArgs q) {
         inv_xm1 = block_batch_invert<QUO_TPB>(xm1, tree, q.prod_inv ? q.prod_inv + blockIdx.x : nullptr);
         if (!live) return;
     }
-    const Fr a = gmem_ld(q.w[0] + i), b = gmem_ld(q.w[1] + i), c = gmem_ld(q.w[2] + i), d = gmem_ld(q.w[3] + i), e = gmem_ld(q.w[4] + i);
+    Fr a = gmem_ld(q.w[0] + i), b = gmem_ld(q.w[1] + i), c = gmem_ld(q.w[2] + i), d = gmem_ld(q.w[3] + i), e = gmem_ld(q.w[4] + i);
+    if constexpr (TAIL) {
+        const Fr xn = q.xn[pt % q.ratio];
+        auto blind = [&](Fr &w, int j) {
+            if (q.w_tail_len[j]) w = w + qmul(xn, quotient_tail_at(q.w_tail[j], q.w_tail_len[j], x));
+        };
+        blind(a, 0), blind(b, 1), blind(c, 2), blind(d, 3), blind(e, 4);
+    }
     const Fr ab = qmul(a, b), cd = qmul(c, d);
     // gate constraint (lines 451-472)
     Fr gate = gmem_ld(q.sel[11] + i) + gmem_ld(q.pi + i);
@@ -172,8 +207,15 @@ __global__ void __launch_bounds__(QUO_TPB) quotient_kernel(QuotientArgs q) {
     }
     gate = gate - qmul(gmem_ld(q.sel[10] + i), e);
     // permutation constraint (lines 473-491): z(X) prod(w + beta k X + gamma) - z(omega X) prod(w + beta sigma + gamma)
-    const Fr zi = gmem_ld(q.z + i);
-    Fr acc1 = zi, acc2 = gmem_ld(q.z + ((i + q.z_next) & (q.pts - 1)));
+    Fr zi = gmem_ld(q.z + i), zw = gmem_ld(q.z + ((i + q.z_next) & (q.pts - 1)));
+    if constexpr (TAIL) {
+        if (q.z_tail_len) {
+            const Fr xn = q.xn[pt % q.ratio];
+            zi = zi + qmul(xn, quotient_tail_at(q.z_tail, q.z_tail_len, x));
+            zw = zw + qmul(xn, quotient_tail_at(q.z_tail, q.z_tail_len, qmul(q.omega_n, x)));
+        }
+    }
+    Fr acc1 = zi, acc2 = zw;
 #pragma unroll
     for (int j = 0; j < 5; j++) {
         const Fr t = wv[j] + q.gamma;

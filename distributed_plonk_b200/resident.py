@@ -14,8 +14,14 @@ evaluations) goes in once; 13 commitments and 10 evaluations come back:
   round 5  linearisation and batch polynomials, two divisions by          557-690
            (X - point), 2 commitments
 
-Out of scope here, as everywhere in this repo: the Fiat-Shamir transcript (challenges are inputs) and the
-blinding scalars (two extra coefficients per wire; `dp_round1` does them for the RPC the worker has).
+prove(..., blind=True) blinds as the reference prover does (dispatcher2.rs:294-361), which makes the proof
+zero-knowledge: every wire gets + (b_0 + b_1 X) * Z_H and z gets + (b_0 + b_1 X + b_2 X^2) * Z_H (dp_poly_blind_dev,
+13 secret scalars drawn inside the library), so they have n + 2 and n + 3 coefficients, and the quotient has degree
+5(n+1)+2 on a satisfied circuit, the degree the reference's split_quot_polys requires.  Round 3 still transforms the
+first n coefficients of each polynomial; the quotient kernel adds x^n * tail(x) for the last 2 or 3 (DESIGN.md 3.4).
+blind=False (the default) leaves the proof unblinded, the computation as before.
+
+Out of scope here, as everywhere in this repo: the Fiat-Shamir transcript (challenges are inputs).
 The proving key (13 selector + 5 sigma polynomials in coefficient form, sigma / identity permutation
 evaluations) stays resident across proofs, as `State` keeps the bases (worker.rs:42-59).
 
@@ -28,6 +34,8 @@ import numpy as np
 
 N_SEL, N_WIRE = 13, 5
 N_COEF = N_SEL + 2 * N_WIRE + 2       # polynomials evaluated on the quotient coset in round 3
+BLIND_WIRE, BLIND_Z = 2, 3            # blinding scalars of each wire (rand(1) * Z_H) and of z (rand(2) * Z_H)
+N_BLIND = N_WIRE * BLIND_WIRE + BLIND_Z
 
 
 class ResidentProver:
@@ -61,11 +69,12 @@ class ResidentProver:
         self.id_eval = buf(N_WIRE * n)
         self.wire_eval = buf(N_WIRE * n)
         self.pub = buf(n)
-        self.wire_coef = [buf(n) for _ in range(N_WIRE)]
-        self.z = buf(n)
+        # coefficient buffers with room for the blinding tails (prove(blind=...)); unblinded, only the first n are used
+        self.wire_coef = [buf(n + BLIND_WIRE) for _ in range(N_WIRE)]
+        self.z = buf(n + BLIND_Z)
         self.quot = buf(m)
-        self.lin = buf(n + 2)
-        self.batch = buf(n + 2)
+        self.lin = buf(n + BLIND_Z)
+        self.batch = buf(n + BLIND_Z)
         self.wit = [buf(n + 2), buf(n + 2)]
         if quotient == "auto":
             quotient = "whole" if self.whole_fits(torch, device, m) else "sliced"
@@ -74,6 +83,7 @@ class ResidentProver:
         # slice buffers are the heads of the whole-domain ones): tools/bench_resident.py times both modes on one prover that way.
         self.big = [buf(m) for _ in range(N_COEF)] if quotient == "whole" else None
         self.slices = [t[:n] for t in self.big] if self.big is not None else [buf(n) for _ in range(N_COEF)]
+        self._srs_checked = False
 
     @classmethod
     def whole_fits(cls, torch, device: str, m: int) -> bool:
@@ -98,45 +108,83 @@ class ResidentProver:
         if self.dev != "cpu":
             self.torch.cuda.current_stream().synchronize()
 
+    def _check_srs(self):
+        """a blinded proof commits z with n + 3 coefficients: the SRS must have that many bases"""
+        if self._srs_checked:
+            return
+        from ._binding import DpError
+        try:
+            self.ctx.get_bases(self.n + BLIND_Z - 1, 1)
+        except DpError as e:
+            raise ValueError(f"a blinded proof of 2^{self.log_n} gates commits polynomials of n + {BLIND_Z} coefficients: the SRS "
+                             f"given to dp_init needs at least {self.n + BLIND_Z} bases") from e
+        self._srs_checked = True
+
     # ---- one proof
-    def prove(self, wire_evals_host, pub_host, ch):
+    def prove(self, wire_evals_host, pub_host, ch, blind=False):
         """wire_evals_host: torch tensor [5n,4] (pinned host memory on a GPU), pub_host [n,4]; ch: dict of the
-        challenges beta, gamma, alpha, zeta, v as raw Fr.  Returns (commitments: list of 13 x 144 B, evals: list)"""
+        challenges beta, gamma, alpha, zeta, v as raw Fr.  Returns (commitments: list of 13 x 144 B, evals: list).
+        blind: False (unblinded), True (the library draws the N_BLIND = 13 blinding scalars from the OS entropy pool) or
+        an [13,4] array of raw Fr below r (wire i takes rows 2i, 2i+1, z rows 10-12; reproducible proofs for tests)"""
         ctx, n, m, log_n, F = self.ctx, self.n, self.m, self.log_n, self.F
         log_m = log_n + 3
         com, P = [], lambda t: t.data_ptr()
+        blinded = blind is not False
+        scalars = None
+        if blinded:
+            self._check_srs()
+            if blind is not True:
+                scalars = np.ascontiguousarray(blind, dtype=np.uint64)
+                if scalars.shape != (N_BLIND, 4):
+                    raise ValueError(f"blind: an array of shape ({N_BLIND}, 4) of raw Fr, True or False, not shape {scalars.shape}")
+        nw, nz = (n + BLIND_WIRE, n + BLIND_Z) if blinded else (n, n)   # coefficients of each wire / of z
         # witness in: the only bulk host->device traffic of the proof
         self.wire_eval.copy_(wire_evals_host, non_blocking=True)
         self.pub.copy_(pub_host, non_blocking=True)
         for i in range(N_WIRE):
-            self.wire_coef[i].copy_(self.wire_eval[i * n:(i + 1) * n])
+            self.wire_coef[i][:n].copy_(self.wire_eval[i * n:(i + 1) * n])
+        if blinded:                                            # the blinding adds to coefficients n, n+1, ...
+            for t in self.wire_coef + [self.z]:
+                t[n:].zero_()
         self._sync()                                           # torch's stream -> the library's streams
         # round 1
         for i in range(N_WIRE):
             ctx.ntt_dev(P(self.wire_coef[i]), log_n, True, False)
-            com.append(ctx.commit_dev(P(self.wire_coef[i]), n))
+            if blinded:
+                ctx.poly_blind_dev(P(self.wire_coef[i]), n, BLIND_WIRE, None if scalars is None else scalars[BLIND_WIRE * i:BLIND_WIRE * (i + 1)])
+            com.append(ctx.commit_dev(P(self.wire_coef[i]), nw))
         # round 2
         ctx.perm_product_dev(P(self.wire_eval), P(self.id_eval), P(self.sig_eval), N_WIRE, n, ch["beta"], ch["gamma"], P(self.z))
         ctx.ntt_dev(P(self.z), log_n, True, False)
-        com.append(ctx.commit_dev(P(self.z), n))
+        if blinded:
+            ctx.poly_blind_dev(P(self.z), n, BLIND_Z, None if scalars is None else scalars[N_WIRE * BLIND_WIRE:])
+        com.append(ctx.commit_dev(P(self.z), nz))
         ctx.ntt_dev(P(self.pub), log_n, True, False)
-        # round 3: 25 coset evaluations on the 8n domain, the quotient evaluations, one coset-iNTT(8n)
+        # round 3: 25 coset evaluations on the 8n domain, the quotient evaluations, one coset-iNTT(8n).  Blinded, the wires
+        # and z are transformed on their first n coefficients and the quotient kernel adds the rest (their tails)
         srcs = self.sel_coef + self.sig_coef + self.wire_coef + [self.z, self.pub]
         qargs = (self.k, ch["alpha"], ch["beta"], ch["gamma"])
+        tails = [(P(t) + 32 * n, BLIND_WIRE) for t in self.wire_coef] + [(P(self.z) + 32 * n, BLIND_Z)] if blinded else None
         if self.quotient == "whole":   # only the n coefficients at the head of each buffer are read
             for dst, src in zip(self.big, srcs):
-                dst[:n].copy_(src)
+                dst[:n].copy_(src[:n])
             self._sync()
             for dst in self.big:
                 ctx.ntt_dev_padded(P(dst), n, log_m, False, True, wait=False)
             b = [P(t) for t in self.big]
-            ctx.quotient_evals_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, P(self.quot))
+            if blinded:
+                ctx.quotient_evals_tail_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, tails, P(self.quot))
+            else:
+                ctx.quotient_evals_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, P(self.quot))
         else:                          # slice k into the same 25 n-point buffers, every k; all of it on the library's stream
             b = [P(t) for t in self.slices]
             for k in range(m // n):
                 for dst, src in zip(b, srcs):
                     ctx.ntt_dev_quot_slice(P(src), n, k, dst, wait=False)
-                ctx.quotient_evals_slice_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, k, P(self.quot))
+                if blinded:
+                    ctx.quotient_evals_slice_tail_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, tails, k, P(self.quot))
+                else:
+                    ctx.quotient_evals_slice_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, k, P(self.quot))
         ctx.ntt_dev(P(self.quot), log_m, True, True)
         chunk = n + 2
         for j in range(N_WIRE):
@@ -144,9 +192,9 @@ class ResidentProver:
         # round 4
         zeta = ch["zeta"]
         zeta_w = F.mul(zeta, F.omega)
-        w_ev = [ctx.poly_eval(P(self.wire_coef[i]), zeta, n) for i in range(N_WIRE)]
+        w_ev = [ctx.poly_eval(P(self.wire_coef[i]), zeta, nw) for i in range(N_WIRE)]
         s_ev = [ctx.poly_eval(P(self.sig_coef[i]), zeta, n) for i in range(N_WIRE - 1)]
-        z_next = ctx.poly_eval(P(self.z), zeta_w, n)
+        z_next = ctx.poly_eval(P(self.z), zeta_w, nz)
         # round 5: the scalar coefficients are host glue (a few dozen field operations), the polynomials stay put
         a, bb, c, d, e = w_ev
         ab, cd = F.mul(a, bb), F.mul(c, d)
@@ -170,18 +218,19 @@ class ResidentProver:
             cur = F.mul(cur, zn2)
         coeffs = [a, bb, c, d, ab, cd, p5(a), p5(bb), p5(c), p5(d), neg(e), one, F.mul(F.mul(ab, cd), e), cz, cs] + qc
         polys = [P(t) for t in self.sel_coef] + [P(self.z), P(self.sig_coef[N_WIRE - 1])] + [P(self.quot) + 32 * j * chunk for j in range(N_WIRE)]
-        lens = [n] * (N_SEL + 2) + [chunk] * N_WIRE
-        ctx.poly_lincomb(polys, np.stack(coeffs), out_len=chunk, lens=lens, out_ptr=P(self.lin))
+        lens = [n] * N_SEL + [nz, n] + [chunk] * N_WIRE
+        lin_len = max(chunk, nz)                               # n + 2, or n + 3 with the blinded z
+        ctx.poly_lincomb(polys, np.stack(coeffs), out_len=lin_len, lens=lens, out_ptr=P(self.lin))
         vs, cur = [], one
         for _ in range(1 + N_WIRE + N_WIRE - 1):
             vs.append(cur)
             cur = F.mul(cur, ch["v"])
         polys = [P(self.lin)] + [P(t) for t in self.wire_coef] + [P(t) for t in self.sig_coef[:-1]]
-        ctx.poly_lincomb(polys, np.stack(vs), out_len=chunk, lens=[chunk] + [n] * (2 * N_WIRE - 1), out_ptr=P(self.batch))
-        ctx.poly_div_linear(P(self.batch), zeta, chunk, P(self.wit[0]))
-        com.append(ctx.commit_dev(P(self.wit[0]), chunk - 1))
-        ctx.poly_div_linear(P(self.z), zeta_w, n, P(self.wit[1]))
-        com.append(ctx.commit_dev(P(self.wit[1]), n - 1))
+        ctx.poly_lincomb(polys, np.stack(vs), out_len=lin_len, lens=[lin_len] + [nw] * N_WIRE + [n] * (N_WIRE - 1), out_ptr=P(self.batch))
+        ctx.poly_div_linear(P(self.batch), zeta, lin_len, P(self.wit[0]))
+        com.append(ctx.commit_dev(P(self.wit[0]), lin_len - 1))
+        ctx.poly_div_linear(P(self.z), zeta_w, nz, P(self.wit[1]))
+        com.append(ctx.commit_dev(P(self.wit[1]), nz - 1))
         return com, w_ev + s_ev + [z_next]
 
 
@@ -244,10 +293,10 @@ def make_bench_prover(ctx, torch, log_n: int, rand_fr, quotient: str = "auto"):
     return pr, (wires, pub, ch)
 
 
-def bench_leg(ctx, torch, log_n: int, rand_fr, timed, steps: int = 3, quotient: str = "auto", prover=None):
+def bench_leg(ctx, torch, log_n: int, rand_fr, timed, steps: int = 3, quotient: str = "auto", prover=None, blind=False):
     """bench.py's e2e_resident: proofs/s of ResidentProver.prove on synthetic data, witness copied from pinned host memory
     inside the timed region.  The prover picks its round-3 layout (quotient="auto") unless told; `prover` = (pr, inputs) of
-    make_bench_prover to time an existing one (tools/bench_resident.py).  Also records the layout and the leg's peak device
+    make_bench_prover to time an existing one (tools/bench_resident.py); `blind` is passed to prove.  Also records the layout and the leg's peak device
     memory: torch's peak plus what the library's pool added (cudaMemGetInfo before and after; the pool keeps what it
     allocates).  Torch's cached free blocks are returned to the device first, so that the layout is chosen on what is free."""
     if prover is None:
@@ -260,7 +309,7 @@ def bench_leg(ctx, torch, log_n: int, rand_fr, timed, steps: int = 3, quotient: 
     out = {}
 
     def step():
-        out["r"] = pr.prove(wires, pub, ch)
+        out["r"] = pr.prove(wires, pub, ch, blind=blind)
 
     dt, _ = timed(step, steps, 1, False)
     com, ev = out["r"]

@@ -223,6 +223,31 @@ int dp_ntt_dev_quot_slice(dp_ctx *ctx, const void *coeffs_dev, size_t n_valid, u
  * All m/n slices = dp_quotient_evals_dev, byte for byte.  Same errors as dp_ntt_dev_quot_slice.                    */
 int dp_quotient_evals_slice_dev(dp_ctx *ctx, const dp_quotient_args *slice_arrays, uint32_t slice, void *out_dev);
 
+/* Round 3 with blinded wires and z (dispatcher2.rs:294-361: each wire + rand(1)*Z_H, z + rand(2)*Z_H).  A blinded
+ * polynomial has n + t coefficients (t <= 3); split it as p = head + X^n * tail, head = its first n coefficients.
+ * The 25 arrays of dp_quotient_args hold the coset evaluations of the heads only (the usual n-coefficient transforms);
+ * the tails are coefficients n, n+1, ... of each wire and of z, device pointers, t of them (0 = not blinded).  The
+ * output is the quotient of the full polynomials.  With every length 0 it equals dp_quotient_evals[_slice]_dev byte
+ * for byte.  DP_E_ARG for a length > 3, a NULL pointer with a length > 0, or a tail that overlaps the output; else the
+ * errors of the entry without tails.                                                                               */
+typedef struct dp_quotient_tails {
+    const void *wires[5];
+    size_t wire_len[5];
+    const void *perm;
+    size_t perm_len;
+} dp_quotient_tails;
+int dp_quotient_evals_tail_dev(dp_ctx *ctx, const dp_quotient_args *dev_arrays, const dp_quotient_tails *tails, void *out_dev);
+int dp_quotient_evals_slice_tail_dev(dp_ctx *ctx, const dp_quotient_args *slice_arrays, const dp_quotient_tails *tails,
+                                     uint32_t slice, void *out_dev);
+
+/* Blinding, as the reference prover does it to every wire (k = 2) and to z (k = 3): coeffs += b(X) * (X^n - 1),
+ * b(X) = b_0 + b_1 X + ... + b_(k-1) X^(k-1), in place on a device buffer of at least n + k Fr (b_j is subtracted
+ * from coefficient j and added to coefficient n + j).  blind: k raw Fr below r on the host (reproducible, for
+ * tests), or NULL: the library draws k secret scalars uniformly below r from the operating system's entropy pool
+ * (getrandom(2)) and they never leave it.  DP_E_ARG for k > 3 or a scalar not below r; DP_E_STATE if the entropy
+ * source is unavailable.                                                                                          */
+int dp_poly_blind_dev(dp_ctx *ctx, void *coeffs_dev, size_t n, uint32_t k, const void *blind);
+
 /* Round 4, DensePolynomial::evaluate (src/dispatcher2.rs:535-548): out32 = sum_j coeffs[j] * point^j */
 int dp_poly_eval(dp_ctx *ctx, const void *coeffs, size_t n, const void *point, void *out32);
 int dp_poly_eval_dev(dp_ctx *ctx, const void *coeffs_dev, size_t n, const void *point, void *out32);

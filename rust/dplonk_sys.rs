@@ -35,6 +35,15 @@ pub struct dp_quotient_args {
     pub gamma: *const u8,
 }
 
+/// coefficients n, n+1, ... of each blinded wire and of z, device pointers, at most 3 each (include/dplonk.h: dp_quotient_tails)
+#[repr(C)]
+pub struct dp_quotient_tails {
+    pub wires: [*const c_void; 5],
+    pub wire_len: [usize; 5],
+    pub perm: *const c_void,
+    pub perm_len: usize,
+}
+
 extern "C" {
     pub fn dp_create(cuda_device: c_int, me: u64, n_workers: u64, out: *mut *mut dp_ctx) -> c_int;
     pub fn dp_destroy(ctx: *mut dp_ctx) -> c_int;
@@ -64,6 +73,11 @@ extern "C" {
                                  wait: c_int) -> c_int;
     pub fn dp_quotient_evals_slice_dev(ctx: *mut dp_ctx, slice_arrays: *const dp_quotient_args, slice: u32,
                                        out_dev: *mut c_void) -> c_int;
+    pub fn dp_quotient_evals_tail_dev(ctx: *mut dp_ctx, dev_arrays: *const dp_quotient_args, tails: *const dp_quotient_tails,
+                                      out_dev: *mut c_void) -> c_int;
+    pub fn dp_quotient_evals_slice_tail_dev(ctx: *mut dp_ctx, slice_arrays: *const dp_quotient_args, tails: *const dp_quotient_tails,
+                                            slice: u32, out_dev: *mut c_void) -> c_int;
+    pub fn dp_poly_blind_dev(ctx: *mut dp_ctx, coeffs_dev: *mut c_void, n: usize, k: u32, blind_kfr: *const u8) -> c_int;
     pub fn dp_peer_arena_create(ctx: *mut dp_ctx, arena_bytes: u64, handle_out: *mut u8) -> c_int;
     pub fn dp_peer_attach(ctx: *mut dp_ctx, peer: u64, handle: *const u8) -> c_int;
     pub fn dp_peer_ready(ctx: *const dp_ctx) -> c_int;

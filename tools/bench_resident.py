@@ -5,10 +5,13 @@ timed alternately (DESIGN.md 3.4).  Prints one JSON line.
 
     python tools/bench_resident.py --log-n 24 --steps 2
     python tools/bench_resident.py --log-n 22 --steps 3            # + e2e_resident_sliced, alternated with whole
+    python tools/bench_resident.py --log-n 24 --zk                 # blinded (e2e_resident_zk) and unblinded, alternated
 
 Before anything is timed: one seeded slice transform (dp_ntt_dev_quot_slice) at a few positions against the oracle's
 O(n) Horner evaluation, and at log_n <= 22 the 13 commitments and 10 evaluations of both layouts compared byte for byte.
-A mismatch exits with code 3.  Set-up as bench.py's (synthetic SRS generated on the GPU, dp_init's own MSM tuning), with
+With --zk, instead of the two layouts: a proof with all-zero blinders must equal the unblinded proof in all 13 commitments
+and 10 evaluations, then blinded proofs (the library draws the 13 scalars) and unblinded ones are timed alternately on one
+prover in its chosen layout.  A mismatch exits with code 3.  Set-up as bench.py's (synthetic SRS generated on the GPU, dp_init's own MSM tuning), with
 nothing else allocated: no schedule buffers, no host-buffer leg, no CPU baseline."""
 from __future__ import annotations
 
@@ -48,7 +51,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--log-n", type=int, default=22, dest="log_n")
     ap.add_argument("--steps", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=2, help="log_n <= 22: alternations of the two layouts")
+    ap.add_argument("--rounds", type=int, default=2, help="alternations of the two layouts (log_n <= 22) or of blinded and unblinded (--zk)")
+    ap.add_argument("--zk", action="store_true", help="time blinded (zero-knowledge) against unblinded proofs instead of the layouts")
     args = ap.parse_args()
 
     import torch
@@ -97,8 +101,26 @@ def main():
         prover = resident.make_bench_prover(ctx, torch, log_n, rand_fr)
         pr, (wires, pub, ch) = prover
         line["chosen"] = pr.quotient
-        modes = ["whole", "sliced"] if log_n <= 22 and pr.quotient == "whole" else [pr.quotient]
-        if len(modes) == 2:
+        modes = ["whole", "sliced"] if log_n <= 22 and pr.quotient == "whole" and not args.zk else [pr.quotient]
+        if args.zk:
+            plain = pr.prove(wires, pub, ch)
+            zero = pr.prove(wires, pub, ch, blind=np.zeros((resident.N_BLIND, 4), dtype=np.uint64))
+            ok = len(plain[0] + plain[1]) == 23 and all(np.array_equal(np.asarray(a), np.asarray(b))
+                                                         for a, b in zip(plain[0] + plain[1], zero[0] + zero[1]))
+            line["verify"]["zero_blinders_equal_unblinded"] = ok
+            if ok:
+                legs = {False: [], True: []}
+                for _ in range(args.rounds):                              # unblinded, blinded, unblinded, blinded, ...
+                    for b in (False, True):
+                        legs[b].append(resident.bench_leg(ctx, torch, log_n, rand_fr, timed, args.steps, prover=prover, blind=b))
+                for b, rs in legs.items():
+                    dt, st = sum(r["steps"] / r["value"] for r in rs), sum(r["steps"] for r in rs)
+                    line["e2e_resident_zk" if b else "e2e_resident"] = dict(rs[-1], value=st / dt, ms_per_step=dt / st * 1e3, steps=st,
+                                                                            values=[r["value"] for r in rs])
+                line["value"] = line["e2e_resident"]["value"]
+                line["zk_cost"] = {"slowdown": round(line["e2e_resident"]["value"] / line["e2e_resident_zk"]["value"] - 1, 4),
+                                   "what": "unblinded proofs/s over blinded proofs/s, minus 1, alternated on one prover"}
+        elif len(modes) == 2:
             outs = {}
             for mode in modes:
                 pr.quotient = mode
@@ -106,7 +128,7 @@ def main():
                 outs[mode] = [np.asarray(x) for x in com + ev]
             ok = len(outs["whole"]) == 23 and all(np.array_equal(a, b) for a, b in zip(outs["whole"], outs["sliced"]))
             line["verify"]["resident_sliced_equals_whole"] = ok
-        if ok:
+        if ok and not args.zk:
             legs = {mode: [] for mode in modes}
             for _ in range(args.rounds if len(modes) == 2 else 1):     # whole, sliced, whole, sliced, ...
                 for mode in modes:
@@ -118,7 +140,8 @@ def main():
                 line[key] = dict(rs[-1], value=st / dt, ms_per_step=dt / st * 1e3, steps=st, values=[r["value"] for r in rs])
             line["value"] = line["e2e_resident"]["value"]
     if not ok:
-        line["error"] = "the sliced resident prover disagrees with the oracle or with the whole-domain prover"
+        line["error"] = ("a proof with zero blinders differs from the unblinded proof" if args.zk and "zero_blinders_equal_unblinded" in line["verify"]
+                         else "the sliced resident prover disagrees with the oracle or with the whole-domain prover")
     print(json.dumps(line), flush=True)
     ctx.close()
     if not ok:
