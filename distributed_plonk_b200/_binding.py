@@ -20,6 +20,7 @@ EXPORTS = [
     "dp_fft_exchange_begin_async", "dp_compute_stream", "dp_fft_dev_p2p_async", "dp_fft1_rows_short", "dp_fft_dev_hint_valid_cols", "dp_ntt_dev_padded", "dp_debug_set_three_pass",
     "dp_ntt_dev_quot_slice", "dp_quotient_evals_slice_dev",
     "dp_poly_blind_dev", "dp_quotient_evals_tail_dev", "dp_quotient_evals_slice_tail_dev",
+    "dp_wire_permutation_scratch_bytes", "dp_wire_permutation_dev", "dp_perm_evals_dev", "dp_witness_gather_dev", "dp_commit_dev_batch",
 ]
 
 
@@ -110,6 +111,11 @@ def bind(cdll: C.CDLL) -> C.CDLL:
         "dp_quotient_evals_tail_dev": (i, [vp, C.POINTER(QuotientArgs), C.POINTER(QuotientTails), vp]),
         "dp_quotient_evals_slice_tail_dev": (i, [vp, C.POINTER(QuotientArgs), C.POINTER(QuotientTails), u32, vp]),
         "dp_poly_blind_dev": (i, [vp, vp, sz, u32, vp]),
+        "dp_wire_permutation_scratch_bytes": (i, [sz, sz, u64, C.POINTER(sz)]),
+        "dp_wire_permutation_dev": (i, [vp, vp, sz, sz, u64, vp, sz, vp]),
+        "dp_perm_evals_dev": (i, [vp, vp, sz, sz, vp, vp, vp]),
+        "dp_witness_gather_dev": (i, [vp, vp, u64, vp, sz, sz, sz, vp, vp]),
+        "dp_commit_dev_batch": (i, [vp, sz, C.POINTER(vp), C.POINTER(sz), vp]),
         "dp_poly_eval": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_eval_dev": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_lincomb": (i, [vp, C.POINTER(vp), C.POINTER(sz), vp, sz, vp, sz]),
@@ -376,6 +382,34 @@ class Context:
         the k scalars from the OS entropy pool and they never leave it"""
         b = np.ascontiguousarray(blind, dtype=np.uint64) if blind is not None else None
         self._ck(self.lib.dp_poly_blind_dev(self.h, coeffs_ptr, n, k, _addr(b) if b is not None else None))
+
+    # ---- circuit preprocessing and the witness gather (device pointers; slot s = wire type * n + gate)
+    def wire_permutation_scratch_bytes(self, num_wire_types: int, n: int, num_vars: int) -> int:
+        b = C.c_size_t()
+        self._ck(self.lib.dp_wire_permutation_scratch_bytes(num_wire_types, n, num_vars, C.byref(b)))
+        return b.value
+
+    def wire_permutation_dev(self, vars_ptr: int, num_wire_types: int, n: int, num_vars: int, scratch_ptr: int, scratch_bytes: int,
+                             succ_ptr: int):
+        """succ[s] = the next slot holding the same variable (wrapping to its first); u32 arrays of num_wire_types * n"""
+        self._ck(self.lib.dp_wire_permutation_dev(self.h, vars_ptr, num_wire_types, n, num_vars, scratch_ptr, scratch_bytes, succ_ptr))
+
+    def perm_evals_dev(self, succ_ptr, num_wire_types: int, n: int, k: np.ndarray, id_ptr: int, sigma_ptr: int):
+        """id[i n + j] = k_i omega^j, sigma[s] = id[succ[s]] (succ_ptr None: sigma = id); k = [num_wire_types, 4] raw Fr"""
+        kk = np.ascontiguousarray(k, dtype=np.uint64)
+        self._ck(self.lib.dp_perm_evals_dev(self.h, succ_ptr, num_wire_types, n, _addr(kk), id_ptr, sigma_ptr))
+
+    def witness_gather_dev(self, witness_ptr: int, num_vars: int, vars_ptr: int, num_wire_types: int, n: int, num_inputs: int,
+                           wires_ptr: int, pub_ptr: int):
+        """wires[s] = witness[vars[s]]; pub[j] = the last wire type's value at gate j < num_inputs, 0 up to n"""
+        self._ck(self.lib.dp_witness_gather_dev(self.h, witness_ptr, num_vars, vars_ptr, num_wire_types, n, num_inputs, wires_ptr, pub_ptr))
+
+    def commit_dev_batch(self, ptrs, lens) -> list:
+        """commit_dev of several device polynomials as one MSM batch; returns [144-byte arrays]"""
+        k = len(ptrs)
+        out = np.zeros((k, G1_PROJECTIVE_BYTES), dtype=np.uint8)
+        self._ck(self.lib.dp_commit_dev_batch(self.h, k, (C.c_void_p * k)(*ptrs), (C.c_size_t * k)(*lens), _addr(out) if k else None))
+        return list(out)
 
     def poly_eval(self, coeffs, point: np.ndarray, n: int | None = None) -> np.ndarray:
         """round 4: p(point); coeffs = [n,4] host array, or a device pointer with n given"""

@@ -14,6 +14,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include "circuit.cuh"
 #include "msm.cuh"
 #include "ntt.cuh"
 #include "perm.cuh"
@@ -2380,6 +2381,216 @@ int dp_perm_product_dev(dp_ctx *ctx, const void *wires_dev, const void *id_dev, 
     memcpy(&be, beta, sizeof be);
     memcpy(&ga, gamma, sizeof ga);
     DP_TRY(perm_product_device(ctx, (const Fr *)wires_dev, (const Fr *)id_dev, (const Fr *)sigma_dev, (uint32_t)num_wire_types, n, be, ga, (Fr *)out_dev));
+    return call_end(ctx, true);
+}
+
+// ------------------------------------------------------------------ circuit preprocessing and witness gather (circuit.cuh)
+// Sort scratch of dp_wire_permutation_dev, offsets in bytes: key / value buffers (one pair for a single radix pass, two to
+// ping-pong between), the digit histograms of every block, their scan's block sums, the id-check flag.
+struct WirePermLayout {
+    uint32_t passes = 0, n_blocks = 0, hist_n = 0, scan_blocks = 0;
+    uint64_t keys[2] = {0, 0}, vals[2] = {0, 0}, hist = 0, bsum = 0, flag = 0, total = 0;
+};
+
+static WirePermLayout wire_perm_layout(uint64_t count, uint64_t num_vars) {
+    WirePermLayout L;
+    uint64_t top = num_vars - 1;                       // largest id; ids are u32
+    if (top > 0xffffffffull) top = 0xffffffffull;
+    uint32_t bits = 0;
+    while (bits < 64 && (top >> bits)) bits++;
+    L.passes = (bits + CIRC_RADIX_BITS - 1) / CIRC_RADIX_BITS;
+    L.n_blocks = (uint32_t)((count + CIRC_TILE - 1) / CIRC_TILE);
+    L.hist_n = CIRC_RADIX * L.n_blocks;
+    L.scan_blocks = (L.hist_n + SCAN_BLOCK - 1) / SCAN_BLOCK;
+    uint64_t off = 0;
+    auto take = [&](uint64_t bytes) {
+        const uint64_t at = off;
+        off += (bytes + 255) & ~(uint64_t)255;
+        return at;
+    };
+    const uint32_t pairs = L.passes < 2 ? L.passes : 2;
+    for (uint32_t p = 0; p < pairs; p++) {
+        L.keys[p] = take(count * sizeof(uint32_t));
+        L.vals[p] = take(count * sizeof(uint32_t));
+    }
+    if (L.passes) {
+        L.hist = take((uint64_t)L.hist_n * sizeof(uint32_t));
+        L.bsum = take((uint64_t)L.scan_blocks * sizeof(uint32_t));
+    }
+    L.flag = take(sizeof(uint32_t));
+    L.total = off;
+    return L;
+}
+
+// *ok = every ids[i] < bound; flag_dev: one u32 of device scratch.  Waits for the answer.
+static int ids_below(dp_ctx *ctx, const uint32_t *ids, uint64_t count, uint64_t bound, uint32_t *flag_dev, bool *ok) {
+    DP_CUDA(ctx, cudaMemsetAsync(flag_dev, 0, sizeof(uint32_t), ctx->stream));
+    uint64_t grid = blocks_for(count, 256);
+    if (grid > (uint64_t)ctx->n_sms * 8) grid = (uint64_t)ctx->n_sms * 8;
+    DP_LAUNCH(circ_check_ids_kernel, dim3((unsigned)(grid ? grid : 1)), dim3(256), 0, ctx->stream, ids, count, bound, flag_dev);
+    ctx->launches++;
+    uint32_t flag = 0;
+    DP_CUDA(ctx, cudaMemcpyAsync(&flag, flag_dev, sizeof flag, cudaMemcpyDeviceToHost, ctx->stream));
+    DP_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    DP_CUDA(ctx, cudaGetLastError());
+    *ok = flag == 0;
+    return DP_OK;
+}
+
+// the arguments every circuit entry shares: after dp_init, 1..5 wire types over the gate domain, slots indexable by u32
+static int circuit_args(dp_ctx *ctx, size_t num_wire_types, size_t n, const char *who) {
+    if (!ctx->inited) return fail(ctx, DP_E_STATE, "%s before dp_init", who);
+    if (num_wire_types < 1 || num_wire_types > 5) return fail(ctx, DP_E_ARG, "%s: %zu wire types (1..5)", who, num_wire_types);
+    if (n != ctx->dom[0].n()) return fail(ctx, DP_E_ARG, "%s: n = %zu is not the gate domain (%llu)", who, n, (unsigned long long)ctx->dom[0].n());
+    if ((uint64_t)num_wire_types * n > 0xffffffffull) return fail(ctx, DP_E_ARG, "%s: %zu slots do not fit 32-bit slot ids", who, num_wire_types * n);
+    return DP_OK;
+}
+
+int dp_wire_permutation_scratch_bytes(size_t num_wire_types, size_t n, uint64_t num_vars, size_t *bytes) {
+    if (!bytes || num_wire_types < 1 || num_wire_types > 5 || n == 0 || num_vars == 0 || (uint64_t)num_wire_types * n > 0xffffffffull)
+        return fail(nullptr, DP_E_ARG, "dp_wire_permutation_scratch_bytes: %zu wire types, n = %zu, %llu variables", num_wire_types, n,
+                    (unsigned long long)num_vars);
+    *bytes = wire_perm_layout((uint64_t)num_wire_types * n, num_vars).total;
+    return DP_OK;
+}
+
+int dp_wire_permutation_dev(dp_ctx *ctx, const uint32_t *vars_dev, size_t num_wire_types, size_t n, uint64_t num_vars, void *scratch_dev,
+                            size_t scratch_bytes, uint32_t *succ_out_dev) {
+    const char *who = "dp_wire_permutation_dev";
+    if (!ctx) return fail(ctx, DP_E_ARG, "%s: NULL context", who);
+    DP_TRY(circuit_args(ctx, num_wire_types, n, who));
+    if (!vars_dev || !scratch_dev || !succ_out_dev) return fail(ctx, DP_E_ARG, "%s: NULL argument", who);
+    if (num_vars == 0) return fail(ctx, DP_E_ARG, "%s: num_vars = 0", who);
+    const uint64_t count = (uint64_t)num_wire_types * n;
+    const WirePermLayout L = wire_perm_layout(count, num_vars);
+    if (scratch_bytes < L.total) return fail(ctx, DP_E_ARG, "%s: %zu scratch bytes, %llu needed", who, scratch_bytes, (unsigned long long)L.total);
+    if (ranges_overlap(vars_dev, count * 4, succ_out_dev, count * 4) || ranges_overlap(vars_dev, count * 4, scratch_dev, L.total) ||
+        ranges_overlap(succ_out_dev, count * 4, scratch_dev, L.total))
+        return fail(ctx, DP_E_ARG, "%s: the variable map, the scratch and the output overlap", who);
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    uint8_t *S = (uint8_t *)scratch_dev;
+    bool ok = false;
+    DP_TRY(ids_below(ctx, vars_dev, count, num_vars, (uint32_t *)(S + L.flag), &ok));
+    if (!ok) return fail(ctx, DP_E_ARG, "%s: a variable id is >= num_vars = %llu", who, (unsigned long long)num_vars);
+    const uint32_t *keys = vars_dev, *vals = nullptr;
+    uint32_t *hist = (uint32_t *)(S + L.hist), *bsum = (uint32_t *)(S + L.bsum);
+    for (uint32_t p = 0; p < L.passes; p++) {
+        uint32_t *ko = (uint32_t *)(S + L.keys[p & 1]), *vo = (uint32_t *)(S + L.vals[p & 1]);
+        const uint32_t shift = p * CIRC_RADIX_BITS;
+        DP_LAUNCH(circ_radix_hist_kernel, dim3(L.n_blocks), dim3(CIRC_TPB), 0, ctx->stream, keys, count, shift, L.n_blocks, hist);
+        DP_LAUNCH(scan_block_sums_kernel, dim3(L.scan_blocks), dim3(SCAN_TPB), 0, ctx->stream, (const uint32_t *)hist, L.hist_n, bsum);
+        DP_LAUNCH(circ_scan_offsets_kernel, dim3(1), dim3(CIRC_TPB), 0, ctx->stream, bsum, L.scan_blocks);
+        DP_LAUNCH(circ_scan_write_kernel, dim3(L.scan_blocks), dim3(SCAN_TPB), 0, ctx->stream, hist, L.hist_n, (const uint32_t *)bsum);
+        DP_LAUNCH(circ_radix_scatter_kernel, dim3(L.n_blocks), dim3(CIRC_TPB), 0, ctx->stream, keys, vals, count, shift,
+                  (const uint32_t *)hist, L.n_blocks, ko, vo);
+        ctx->launches += 5;
+        DP_CUDA(ctx, cudaGetLastError());
+        keys = ko;
+        vals = vo;
+    }
+    DP_LAUNCH(circ_successor_kernel, dim3(blocks_for(count, 256)), dim3(256), 0, ctx->stream, keys, vals, count, succ_out_dev);
+    ctx->launches++;
+    DP_CUDA(ctx, cudaGetLastError());
+    return call_end(ctx, true);
+}
+
+int dp_perm_evals_dev(dp_ctx *ctx, const uint32_t *succ_dev, size_t num_wire_types, size_t n, const void *k, void *id_out_dev,
+                      void *sigma_out_dev) {
+    const char *who = "dp_perm_evals_dev";
+    if (!ctx) return fail(ctx, DP_E_ARG, "%s: NULL context", who);
+    DP_TRY(circuit_args(ctx, num_wire_types, n, who));
+    if (!k || !id_out_dev || !sigma_out_dev) return fail(ctx, DP_E_ARG, "%s: NULL argument", who);
+    const uint64_t count = (uint64_t)num_wire_types * n;
+    if (ranges_overlap(id_out_dev, count * 32, sigma_out_dev, count * 32) ||
+        (succ_dev && (ranges_overlap(succ_dev, count * 4, id_out_dev, count * 32) || ranges_overlap(succ_dev, count * 4, sigma_out_dev, count * 32))))
+        return fail(ctx, DP_E_ARG, "%s: the successor map and the outputs overlap", who);
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    if (succ_dev) {
+        Scratch tmp(ctx->pool);
+        uint32_t *flag = tmp.get<uint32_t>(1);
+        if (!flag) return fail(ctx, DP_E_OOM, "%s flag", who);
+        bool ok = false;
+        DP_TRY(ids_below(ctx, succ_dev, count, count, flag, &ok));
+        if (!ok) return fail(ctx, DP_E_ARG, "%s: a successor slot is >= num_wire_types * n = %llu", who, (unsigned long long)count);
+    }
+    CircK kk;
+    memset((void *)&kk, 0, sizeof kk);
+    memcpy(kk.k, k, num_wire_types * sizeof(Fr));
+    DP_LAUNCH(circ_perm_evals_kernel, dim3(blocks_for(count, 256)), dim3(256), 0, ctx->stream, succ_dev, count, ctx->dom[0].log_n,
+              (const Fr *)ctx->dom[0].H, kk, (Fr *)id_out_dev, (Fr *)sigma_out_dev);
+    ctx->launches++;
+    DP_CUDA(ctx, cudaGetLastError());
+    return call_end(ctx, true);
+}
+
+int dp_witness_gather_dev(dp_ctx *ctx, const void *witness_dev, uint64_t num_vars, const uint32_t *vars_dev, size_t num_wire_types, size_t n,
+                          size_t num_inputs, void *wires_out_dev, void *pub_out_dev) {
+    const char *who = "dp_witness_gather_dev";
+    if (!ctx) return fail(ctx, DP_E_ARG, "%s: NULL context", who);
+    DP_TRY(circuit_args(ctx, num_wire_types, n, who));
+    if (!witness_dev || !vars_dev || !wires_out_dev || !pub_out_dev) return fail(ctx, DP_E_ARG, "%s: NULL argument", who);
+    if (num_vars == 0) return fail(ctx, DP_E_ARG, "%s: num_vars = 0", who);
+    if (num_inputs > n) return fail(ctx, DP_E_ARG, "%s: %zu public inputs > n = %zu", who, num_inputs, n);
+    const uint64_t count = (uint64_t)num_wire_types * n;
+    const uint64_t wit_bytes = (num_vars < ((uint64_t)1 << 32) ? num_vars : ((uint64_t)1 << 32)) * 32;   // ids are u32
+    if (ranges_overlap(wires_out_dev, count * 32, witness_dev, wit_bytes) || ranges_overlap(wires_out_dev, count * 32, vars_dev, count * 4) ||
+        ranges_overlap(wires_out_dev, count * 32, pub_out_dev, n * 32) || ranges_overlap(pub_out_dev, n * 32, witness_dev, wit_bytes) ||
+        ranges_overlap(pub_out_dev, n * 32, vars_dev, count * 4))
+        return fail(ctx, DP_E_ARG, "%s: an output overlaps an input or the other output", who);
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    uint32_t *flag = tmp.get<uint32_t>(1);
+    if (!flag) return fail(ctx, DP_E_OOM, "%s flag", who);
+    bool ok = false;
+    DP_TRY(ids_below(ctx, vars_dev, count, num_vars, flag, &ok));
+    if (!ok) return fail(ctx, DP_E_ARG, "%s: a variable id is >= num_vars = %llu", who, (unsigned long long)num_vars);
+    DP_LAUNCH(circ_gather_kernel, dim3(blocks_for(count, 256)), dim3(256), 0, ctx->stream, (const Fr *)witness_dev, vars_dev, count, (uint64_t)n,
+              (uint64_t)(num_wire_types - 1) * n, (uint64_t)num_inputs, (Fr *)wires_out_dev, (Fr *)pub_out_dev);
+    ctx->launches++;
+    DP_CUDA(ctx, cudaGetLastError());
+    return call_end(ctx, true);
+}
+
+int dp_commit_dev_batch(dp_ctx *ctx, size_t n_jobs, void *const *coeffs_dev, const size_t *lens, void *outs144) {
+    const char *who = "dp_commit_dev_batch";
+    if (!ctx || (n_jobs && (!coeffs_dev || !lens || !outs144))) return fail(ctx, DP_E_ARG, "%s: NULL argument", who);
+    if (!ctx->inited) return fail(ctx, DP_E_STATE, "%s before dp_init", who);
+    for (size_t j = 0; j < n_jobs; j++) {
+        if (lens[j] && !coeffs_dev[j]) return fail(ctx, DP_E_ARG, "%s: polynomial %zu is NULL", who, j);
+        if (lens[j] > ctx->n_bases) return fail(ctx, DP_E_ARG, "%s: polynomial %zu has %zu coefficients > %llu bases", who, j, lens[j],
+                                                (unsigned long long)ctx->n_bases);
+    }
+    if (n_jobs == 0) return DP_OK;
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    G1JacobianOut *od = tmp.get<G1JacobianOut>(n_jobs);
+    if (!od) return fail(ctx, DP_E_OOM, "%s outputs", who);
+    // into_repr in place (the MSM takes canonical scalars), one MSM batch, back to Montgomery form: no n-sized scratch per job
+    for (size_t j = 0; j < n_jobs; j++)
+        if (lens[j]) {
+            DP_LAUNCH(fr_into_repr_kernel, dim3(blocks_for(lens[j], 256)), dim3(256), 0, ctx->stream, (const Fr *)coeffs_dev[j],
+                      (Fr *)coeffs_dev[j], (uint64_t)lens[j], (uint64_t)lens[j]);
+            ctx->launches++;
+        }
+    std::vector<uint64_t> starts(n_jobs, 0), ends(lens, lens + n_jobs);
+    std::vector<void *> outs(n_jobs);
+    for (size_t j = 0; j < n_jobs; j++) outs[j] = od + j;
+    const int rc = dp_msm_dev_batch(ctx, n_jobs, starts.data(), ends.data(), (const void *const *)coeffs_dev, lens, outs.data());
+    for (size_t j = 0; j < n_jobs; j++)
+        if (lens[j]) {
+            DP_LAUNCH(fr_to_mont_kernel, dim3(blocks_for(lens[j], 256)), dim3(256), 0, ctx->stream, (Fr *)coeffs_dev[j], (uint64_t)lens[j]);
+            ctx->launches++;
+        }
+    DP_CUDA(ctx, cudaGetLastError());
+    if (rc != DP_OK) {
+        DP_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        return rc;
+    }
+    DP_CUDA(ctx, cudaMemcpyAsync(outs144, od, n_jobs * sizeof(G1JacobianOut), cudaMemcpyDeviceToHost, ctx->stream));
     return call_end(ctx, true);
 }
 

@@ -84,6 +84,7 @@ class ResidentProver:
         self.big = [buf(m) for _ in range(N_COEF)] if quotient == "whole" else None
         self.slices = [t[:n] for t in self.big] if self.big is not None else [buf(n) for _ in range(N_COEF)]
         self._srs_checked = False
+        self.vars = self.witness = None                       # load_circuit: the variable map and the witness buffer
 
     @classmethod
     def whole_fits(cls, torch, device: str, m: int) -> bool:
@@ -103,6 +104,64 @@ class ResidentProver:
         self.sig_eval.copy_(t.as_tensor(np.concatenate(sig_eval).view(np.int64)))
         self.id_eval.copy_(t.as_tensor(np.concatenate(id_eval).view(np.int64)))
         self.k = np.ascontiguousarray(k, dtype=np.uint64)
+
+    def load_circuit(self, selector_evals, wire_vars, num_vars: int, k, num_inputs: int):
+        """the proving key from a circuit, on the device: selector_evals [13][n,4] raw Fr (evaluations over the gate domain),
+        wire_vars [5n] u32 variable ids in slot order (wire type * n + gate), num_vars, the coset representatives k[5] and
+        the number of public inputs (the output wires of the first num_inputs gates).  Builds the wire permutation, the
+        identity and sigma evaluations, the 13 + 5 coefficient forms (in-place iNTTs) and commits all 18 in one MSM batch
+        (one per polynomial in the sliced layout, where memory is short).
+        The variable map and a num_vars-entry witness buffer stay resident for prove_witness.  Returns (verifying-key
+        commitments: 13 selector + 5 sigma, 144 B each; k).  self.load_ms: milliseconds of each step (host clock; each
+        library call returns when its kernels are done)."""
+        import time
+        t, ctx, n, P = self.torch, self.ctx, self.n, lambda x: x.data_ptr()
+        wire_vars = np.ascontiguousarray(wire_vars, dtype=np.uint32)
+        if wire_vars.shape != (N_WIRE * n,):
+            raise ValueError(f"wire_vars: {N_WIRE * n} u32 variable ids, not shape {wire_vars.shape}")
+        if not 0 <= num_inputs <= n:
+            raise ValueError(f"num_inputs = {num_inputs} outside 0..n")
+        self.k = np.ascontiguousarray(k, dtype=np.uint64)
+        for dst, src in zip(self.sel_coef, list(selector_evals)):
+            dst.copy_(t.as_tensor(np.ascontiguousarray(src).view(np.int64)))
+        self.vars = t.as_tensor(wire_vars.view(np.int32)).to(self.dev)
+        self.num_vars, self.num_inputs = int(num_vars), int(num_inputs)
+        self.witness = None
+        self._sync()
+        ms = {}
+        t0 = time.perf_counter()
+        scratch_bytes = ctx.wire_permutation_scratch_bytes(N_WIRE, n, self.num_vars)
+        scratch = t.empty(scratch_bytes, dtype=t.uint8, device=self.dev)
+        succ = t.empty(N_WIRE * n, dtype=t.int32, device=self.dev)
+        ctx.wire_permutation_dev(P(self.vars), N_WIRE, n, self.num_vars, P(scratch), scratch_bytes, P(succ))
+        t1 = time.perf_counter()
+        ms["wire_permutation"] = (t1 - t0) * 1e3
+        del scratch
+        ctx.perm_evals_dev(P(succ), N_WIRE, n, self.k, P(self.id_eval), P(self.sig_eval))
+        t2 = time.perf_counter()
+        ms["perm_evals"] = (t2 - t1) * 1e3
+        del succ
+        if self.dev != "cpu":
+            t.cuda.empty_cache()                              # the sort scratch goes back to the device, not to torch's cache
+        for i in range(N_WIRE):
+            self.sig_coef[i].copy_(self.sig_eval[i * n:(i + 1) * n])
+        self._sync()
+        t3 = time.perf_counter()
+        polys = self.sel_coef + self.sig_coef
+        for p in polys:
+            ctx.ntt_dev(P(p), self.log_n, True, False)
+        t4 = time.perf_counter()
+        ms["intt"] = (t4 - t3) * 1e3
+        # one MSM batch of all 18 holds every job's sort scratch at once: that fits beside the whole-domain layout, which is
+        # only chosen with memory to spare; a sliced prover (2^23, 2^24 gates) commits one polynomial per batch
+        group = len(polys) if self.quotient == "whole" else 1
+        vk = []
+        for g0 in range(0, len(polys), group):
+            vk += ctx.commit_dev_batch([P(p) for p in polys[g0:g0 + group]], [n] * len(polys[g0:g0 + group]))
+        ms["commit"] = (time.perf_counter() - t4) * 1e3
+        self.witness = t.zeros((self.num_vars, 4), dtype=t.int64, device=self.dev)
+        self.load_ms = ms
+        return vk, self.k
 
     def _sync(self):
         if self.dev != "cpu":
@@ -126,9 +185,32 @@ class ResidentProver:
         challenges beta, gamma, alpha, zeta, v as raw Fr.  Returns (commitments: list of 13 x 144 B, evals: list).
         blind: False (unblinded), True (the library draws the N_BLIND = 13 blinding scalars from the OS entropy pool) or
         an [13,4] array of raw Fr below r (wire i takes rows 2i, 2i+1, z rows 10-12; reproducible proofs for tests)"""
-        ctx, n, m, log_n, F = self.ctx, self.n, self.m, self.log_n, self.F
-        log_m = log_n + 3
-        com, P = [], lambda t: t.data_ptr()
+        blinded, scalars = self._blinding(blind)
+        # witness in: the only bulk host->device traffic of the proof
+        self.wire_eval.copy_(wire_evals_host, non_blocking=True)
+        self.pub.copy_(pub_host, non_blocking=True)
+        return self._rounds(ch, blinded, scalars)
+
+    def prove_witness(self, witness_host, ch, blind=False):
+        """prove() from the circuit given to load_circuit: witness_host = torch tensor [num_vars,4] raw Fr (pinned host
+        memory on a GPU), the proof's only bulk host->device copy; the wire and public-input evaluations are gathered on the
+        device (dp_witness_gather_dev), then the rounds run exactly as in prove().  Returns (commitments, evals, public
+        inputs [num_inputs,4] - what the verifier needs besides the proof)"""
+        if self.vars is None:
+            raise ValueError("prove_witness needs a circuit: call load_circuit first")
+        if tuple(witness_host.shape) != (self.num_vars, 4):
+            raise ValueError(f"witness: shape ({self.num_vars}, 4), not {tuple(witness_host.shape)}")
+        blinded, scalars = self._blinding(blind)
+        self.witness.copy_(witness_host, non_blocking=True)
+        self._sync()                                           # torch's stream -> the library's stream
+        P = lambda t: t.data_ptr()
+        self.ctx.witness_gather_dev(P(self.witness), self.num_vars, P(self.vars), N_WIRE, self.n, self.num_inputs, P(self.wire_eval), P(self.pub))
+        pub = self.pub[:self.num_inputs].cpu().numpy().view(np.uint64).copy()
+        com, evals = self._rounds(ch, blinded, scalars)
+        return com, evals, pub
+
+    def _blinding(self, blind):
+        """(blinded, scalars or None) from prove's `blind` argument"""
         blinded = blind is not False
         scalars = None
         if blinded:
@@ -137,10 +219,14 @@ class ResidentProver:
                 scalars = np.ascontiguousarray(blind, dtype=np.uint64)
                 if scalars.shape != (N_BLIND, 4):
                     raise ValueError(f"blind: an array of shape ({N_BLIND}, 4) of raw Fr, True or False, not shape {scalars.shape}")
+        return blinded, scalars
+
+    def _rounds(self, ch, blinded, scalars):
+        """rounds 1-5 from the wire and public-input evaluations in self.wire_eval / self.pub"""
+        ctx, n, m, log_n, F = self.ctx, self.n, self.m, self.log_n, self.F
+        log_m = log_n + 3
+        com, P = [], lambda t: t.data_ptr()
         nw, nz = (n + BLIND_WIRE, n + BLIND_Z) if blinded else (n, n)   # coefficients of each wire / of z
-        # witness in: the only bulk host->device traffic of the proof
-        self.wire_eval.copy_(wire_evals_host, non_blocking=True)
-        self.pub.copy_(pub_host, non_blocking=True)
         for i in range(N_WIRE):
             self.wire_coef[i][:n].copy_(self.wire_eval[i * n:(i + 1) * n])
         if blinded:                                            # the blinding adds to coefficients n, n+1, ...
@@ -291,6 +377,32 @@ def make_bench_prover(ctx, torch, log_n: int, rand_fr, quotient: str = "auto"):
     pub = rand_fr(n).cpu().pin_memory()
     ch = {name: F.from_u64(v) for name, v in (("beta", 0xB17A), ("gamma", 0x6A33A), ("alpha", 0xA1FA), ("zeta", 0x2E7A), ("v", 0x55))}
     return pr, (wires, pub, ch)
+
+
+def bench_circuit_inputs(log_n: int, num_vars: int, seed: int = 0xC1C):
+    """a synthetic variable map: slots on uniform random variables 1..num_vars-1, except the last n/8 gates, whose five wires
+    all hold variable 0 - the one large shared variable that padding a circuit to a power of two produces"""
+    n = 1 << log_n
+    rng = np.random.default_rng(seed)
+    wire_vars = rng.integers(1, max(num_vars, 2), size=(N_WIRE, n), dtype=np.uint32) if num_vars > 1 else np.zeros((N_WIRE, n), dtype=np.uint32)
+    wire_vars[:, n - n // 8:] = 0
+    return wire_vars.reshape(-1)
+
+
+def make_bench_circuit(ctx, torch, log_n: int, rand_fr, num_vars: int | None = None, quotient: str = "auto", num_inputs: int = 16):
+    """a ResidentProver preprocessed from a synthetic circuit (load_circuit): random selector evaluations, the variable map
+    of bench_circuit_inputs with num_vars variables (default 4n), k = (1, 7, 13, 17, 23); the witness (random, so the circuit
+    is not satisfied, which changes nothing about the work) in pinned host memory.  Returns (prover, vk, (witness, ch))"""
+    n = 1 << log_n
+    num_vars = 4 * n if num_vars is None else num_vars
+    F = NumpyField(log_n)
+    pr = ResidentProver(ctx, torch, log_n, "cuda", F, quotient=quotient)
+    sel = [rand_fr(n).cpu().numpy().view(np.uint64) for _ in range(N_SEL)]
+    k = np.stack([F.from_u64(v) for v in (1, 7, 13, 17, 23)])
+    vk, _ = pr.load_circuit(sel, bench_circuit_inputs(log_n, num_vars), num_vars, k, num_inputs)
+    witness = rand_fr(num_vars).cpu().pin_memory()
+    ch = {name: F.from_u64(v) for name, v in (("beta", 0xB17A), ("gamma", 0x6A33A), ("alpha", 0xA1FA), ("zeta", 0x2E7A), ("v", 0x55))}
+    return pr, vk, (witness, ch)
 
 
 def bench_leg(ctx, torch, log_n: int, rand_fr, timed, steps: int = 3, quotient: str = "auto", prover=None, blind=False):

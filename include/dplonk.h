@@ -184,6 +184,36 @@ int dp_perm_product(dp_ctx *ctx, const void *wires, const void *id_perm, const v
 int dp_perm_product_dev(dp_ctx *ctx, const void *wires_dev, const void *id_dev, const void *sigma_dev, size_t num_wire_types, size_t n,
                         const void *beta, const void *gamma, void *out_dev);
 
+/* ---- circuit preprocessing and the witness gather, on the device --------------------------------
+ * What jf-plonk's preprocessing and the dispatcher build on the CPU before round 1 (dispatcher2.rs:299, 337-342, 382-403).
+ * A slot is s = i*n + j (wire type i, gate j), the indexing of wire_permutation[i*n + j].  vars_dev: num_wire_types*n u32
+ * variable ids, slot order.  n must be the gate domain given to dp_init, num_wire_types 1..5.  Every entry returns
+ * DP_E_STATE before dp_init and DP_E_ARG for n != the gate domain, num_wire_types outside 1..5, num_vars == 0, a variable
+ * id >= num_vars, NULL or overlapping buffers; out-of-range ids are found by a check kernel, never read.               */
+/* size of the scratch dp_wire_permutation_dev needs (about 16.5 B per slot when num_vars > 256)                     */
+int dp_wire_permutation_scratch_bytes(size_t num_wire_types, size_t n, uint64_t num_vars, size_t *bytes);
+/* succ_out_dev[s] = the next slot, in increasing slot order, holding the same variable as s; the last slot of a variable
+ * maps to its first (the cycles of jf-relation's compute_wire_permutation).  A stable radix sort of the slots by
+ * variable, ceil(bits(num_vars - 1) / 8) passes, in the caller's scratch (DP_E_ARG when smaller than
+ * dp_wire_permutation_scratch_bytes says).                                                                          */
+int dp_wire_permutation_dev(dp_ctx *ctx, const uint32_t *vars_dev, size_t num_wire_types, size_t n, uint64_t num_vars, void *scratch_dev,
+                            size_t scratch_bytes, uint32_t *succ_out_dev);
+/* id_out_dev[i*n + j] = k[i] * omega_n^j and sigma_out_dev[s] = id[succ_dev[s]] (dispatcher2.rs:340-342), both
+ * num_wire_types*n raw Fr; succ_dev NULL: sigma = id.  k: num_wire_types raw Fr, host.  A host that already holds
+ * jf-plonk's wire_permutation passes it here as flat slots (wire * n + gate).  DP_E_ARG for a slot >= num_wire_types*n.
+ * The permutation argument is sound only when succ_dev is a permutation; that is not checked.                       */
+int dp_perm_evals_dev(dp_ctx *ctx, const uint32_t *succ_dev, size_t num_wire_types, size_t n, const void *k, void *id_out_dev,
+                      void *sigma_out_dev);
+/* wires_out_dev[s] = witness_dev[vars_dev[s]] (num_wire_types*n raw Fr) and pub_out_dev[j] = the last wire type's value
+ * at gate j for j < num_inputs, 0 up to n (the public input: the output wire of the first num_inputs gates, zero-padded
+ * to n as the prover's pub_input).  witness_dev: num_vars raw Fr.  DP_E_ARG also for num_inputs > n.               */
+int dp_witness_gather_dev(dp_ctx *ctx, const void *witness_dev, uint64_t num_vars, const uint32_t *vars_dev, size_t num_wire_types,
+                          size_t n, size_t num_inputs, void *wires_out_dev, void *pub_out_dev);
+/* dp_commit_dev of n_jobs device polynomials as one MSM batch (the joined commitments of a verifying key): outs144 =
+ * n_jobs x 144 B, host.  Each coefficient buffer is converted to canonical form in place for the MSM and restored
+ * before the call returns, so no n-sized scratch is needed per job.  DP_E_ARG for lens[j] > the number of bases.    */
+int dp_commit_dev_batch(dp_ctx *ctx, size_t n_jobs, void *const *coeffs_dev, const size_t *lens, void *outs144);
+
 /* ---- "next" row (SURVEY.md §8f-1): rounds 3-5 of Prover::prove on polynomials resident on the worker
  *
  * The reference declares round3 / round4 / round5 RPCs (hello_world.capnp:26-44) but never implements

@@ -78,6 +78,16 @@ extern "C" {
     pub fn dp_quotient_evals_slice_tail_dev(ctx: *mut dp_ctx, slice_arrays: *const dp_quotient_args, tails: *const dp_quotient_tails,
                                             slice: u32, out_dev: *mut c_void) -> c_int;
     pub fn dp_poly_blind_dev(ctx: *mut dp_ctx, coeffs_dev: *mut c_void, n: usize, k: u32, blind_kfr: *const u8) -> c_int;
+    pub fn dp_wire_permutation_scratch_bytes(num_wire_types: usize, n: usize, num_vars: u64, bytes: *mut usize) -> c_int;
+    pub fn dp_wire_permutation_dev(ctx: *mut dp_ctx, vars_dev: *const u32, num_wire_types: usize, n: usize, num_vars: u64,
+                                   scratch_dev: *mut c_void, scratch_bytes: usize, succ_out_dev: *mut u32) -> c_int;
+    pub fn dp_perm_evals_dev(ctx: *mut dp_ctx, succ_dev: *const u32, num_wire_types: usize, n: usize, k: *const u8,
+                             id_out_dev: *mut c_void, sigma_out_dev: *mut c_void) -> c_int;
+    pub fn dp_witness_gather_dev(ctx: *mut dp_ctx, witness_dev: *const c_void, num_vars: u64, vars_dev: *const u32,
+                                 num_wire_types: usize, n: usize, num_inputs: usize, wires_out_dev: *mut c_void,
+                                 pub_out_dev: *mut c_void) -> c_int;
+    pub fn dp_commit_dev_batch(ctx: *mut dp_ctx, n_jobs: usize, coeffs_dev: *const *mut c_void, lens: *const usize,
+                               outs144: *mut u8) -> c_int;
     pub fn dp_peer_arena_create(ctx: *mut dp_ctx, arena_bytes: u64, handle_out: *mut u8) -> c_int;
     pub fn dp_peer_attach(ctx: *mut dp_ctx, peer: u64, handle: *const u8) -> c_int;
     pub fn dp_peer_ready(ctx: *const dp_ctx) -> c_int;
