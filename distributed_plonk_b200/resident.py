@@ -21,7 +21,11 @@ zero-knowledge: every wire gets + (b_0 + b_1 X) * Z_H and z gets + (b_0 + b_1 X 
 first n coefficients of each polynomial; the quotient kernel adds x^n * tail(x) for the last 2 or 3 (DESIGN.md 3.4).
 blind=False (the default) leaves the proof unblinded, the computation as before.
 
-Out of scope here, as everywhere in this repo: the Fiat-Shamir transcript (challenges are inputs).
+prove_circuit derives the challenges itself: a Fiat-Shamir transcript (transcript.py: merlin over Strobe-128 / Keccak, fed
+what the reference's FakeStandardTranscript feeds it, dispatcher2.rs:44-154) of the verifying key, the public inputs and
+each round's commitments and evaluations, so it returns a Proof (proof.py) that a PLONK verifier accepts; blinded by
+default.  The hashing is host work on a few kilobytes; the verifying-key prefix is hashed once per load_circuit.
+prove and prove_witness still take the challenges as inputs (tests, benchmarks), and make the same library calls.
 The proving key (13 selector + 5 sigma polynomials in coefficient form, sigma / identity permutation
 evaluations) stays resident across proofs, as `State` keeps the bases (worker.rs:42-59).
 
@@ -31,6 +35,9 @@ library under test is the kernel-logic emulator, whose "device" memory is host m
 from __future__ import annotations
 
 import numpy as np
+
+from .proof import Proof, VerifyingKey, fr_from_int, fr_to_int, point_from_jacobian
+from .transcript import PlonkTranscript
 
 N_SEL, N_WIRE = 13, 5
 N_COEF = N_SEL + 2 * N_WIRE + 2       # polynomials evaluated on the quotient coset in round 3
@@ -85,6 +92,8 @@ class ResidentProver:
         self.slices = [t[:n] for t in self.big] if self.big is not None else [buf(n) for _ in range(N_COEF)]
         self._srs_checked = False
         self.vars = self.witness = None                       # load_circuit: the variable map and the witness buffer
+        self.vk = self._vk_transcript = None                  # load_circuit: the verifying key, the transcript after it
+        self.last_challenges, self.last_transcript_ms = None, None
 
     @classmethod
     def whole_fits(cls, torch, device: str, m: int) -> bool:
@@ -158,10 +167,23 @@ class ResidentProver:
         vk = []
         for g0 in range(0, len(polys), group):
             vk += ctx.commit_dev_batch([P(p) for p in polys[g0:g0 + group]], [n] * len(polys[g0:g0 + group]))
-        ms["commit"] = (time.perf_counter() - t4) * 1e3
+        t5 = time.perf_counter()
+        ms["commit"] = (t5 - t4) * 1e3
         self.witness = t.zeros((self.num_vars, 4), dtype=t.int64, device=self.dev)
+        # the verifying key as a verifier sees it, and the transcript after it: the same prefix for every proof
+        pts = [point_from_jacobian(c) for c in vk]
+        self.vk = VerifyingKey(n, self.num_inputs, [fr_to_int(x) for x in self.k], pts[:N_SEL], pts[N_SEL:])
+        self._vk_transcript = PlonkTranscript()
+        self._vk_transcript.append_vk(self.vk)
+        ms["vk_transcript"] = (time.perf_counter() - t5) * 1e3
         self.load_ms = ms
         return vk, self.k
+
+    def verifying_key(self) -> VerifyingKey:
+        """the verifying key of the circuit given to load_circuit"""
+        if self.vk is None:
+            raise ValueError("no verifying key: call load_circuit first")
+        return self.vk
 
     def _sync(self):
         if self.dev != "cpu":
@@ -189,7 +211,7 @@ class ResidentProver:
         # witness in: the only bulk host->device traffic of the proof
         self.wire_eval.copy_(wire_evals_host, non_blocking=True)
         self.pub.copy_(pub_host, non_blocking=True)
-        return self._rounds(ch, blinded, scalars)
+        return self._rounds(lambda stage, outputs: ch, blinded, scalars)
 
     def prove_witness(self, witness_host, ch, blind=False):
         """prove() from the circuit given to load_circuit: witness_host = torch tensor [num_vars,4] raw Fr (pinned host
@@ -201,13 +223,60 @@ class ResidentProver:
         if tuple(witness_host.shape) != (self.num_vars, 4):
             raise ValueError(f"witness: shape ({self.num_vars}, 4), not {tuple(witness_host.shape)}")
         blinded, scalars = self._blinding(blind)
+        pub = self._gather(witness_host)
+        com, evals = self._rounds(lambda stage, outputs: ch, blinded, scalars)
+        return com, evals, pub
+
+    def prove_circuit(self, witness_host, blind=True):
+        """a proof of the circuit given to load_circuit that a PLONK verifier accepts: the challenges come from the
+        transcript (PlonkTranscript over merlin) of the verifying key, the public inputs and each round's commitments and
+        evaluations, as in the reference prover (dispatcher2.rs:239-243, 322-328, 357-362, 533-544, 556-560, 634).
+        witness_host as in prove_witness; blind as in prove, True by default, because a proof for a verifier should be
+        zero-knowledge.  Returns (Proof, public inputs as canonical ints).  Leaves the challenges in self.last_challenges
+        (raw Fr, the dict prove_witness takes) and the host time spent in the transcript - point conversions, hashing -
+        in self.last_transcript_ms"""
+        if self._vk_transcript is None:
+            raise ValueError("prove_circuit needs a circuit: call load_circuit first")
+        if tuple(witness_host.shape) != (self.num_vars, 4):
+            raise ValueError(f"witness: shape ({self.num_vars}, 4), not {tuple(witness_host.shape)}")
+        import time
+        blinded, scalars = self._blinding(blind)
+        pub = self._gather(witness_host)
+        t0 = time.perf_counter()
+        pub_int = [fr_to_int(v) for v in pub]
+        tr = self._vk_transcript.clone()
+        tr.append_pub_input(pub_int)
+        clock = [time.perf_counter() - t0]
+
+        def challenges(stage, outputs):
+            t1 = time.perf_counter()
+            if stage == "evals":
+                ev = [fr_to_int(v) for v in outputs]
+                tr.append_proof_evaluations(ev[:N_WIRE], ev[N_WIRE:2 * N_WIRE - 1], ev[-1])
+            else:
+                tr.append_commitments({"wires": b"witness_poly_comms", "perm": b"perm_poly_comms", "quot": b"quot_poly_comms"}[stage],
+                                      [point_from_jacobian(c) for c in outputs])
+            names = {"wires": ("beta", "gamma"), "perm": ("alpha",), "quot": ("zeta",), "evals": ("v",)}[stage]
+            out = {name: fr_from_int(tr.get_and_append_challenge(name.encode())) for name in names}
+            derived.update(out)
+            clock[0] += time.perf_counter() - t1
+            return out
+
+        derived = {}
+        com, evals = self._rounds(challenges, blinded, scalars)
+        t2 = time.perf_counter()
+        proof = Proof.from_raw(com, evals)
+        self.last_transcript_ms = (clock[0] + time.perf_counter() - t2) * 1e3
+        self.last_challenges = derived
+        return proof, pub_int
+
+    def _gather(self, witness_host):
+        """the witness in, the wire and public-input evaluations gathered on the device; returns the public inputs"""
         self.witness.copy_(witness_host, non_blocking=True)
         self._sync()                                           # torch's stream -> the library's stream
         P = lambda t: t.data_ptr()
         self.ctx.witness_gather_dev(P(self.witness), self.num_vars, P(self.vars), N_WIRE, self.n, self.num_inputs, P(self.wire_eval), P(self.pub))
-        pub = self.pub[:self.num_inputs].cpu().numpy().view(np.uint64).copy()
-        com, evals = self._rounds(ch, blinded, scalars)
-        return com, evals, pub
+        return self.pub[:self.num_inputs].cpu().numpy().view(np.uint64).copy()
 
     def _blinding(self, blind):
         """(blinded, scalars or None) from prove's `blind` argument"""
@@ -221,8 +290,11 @@ class ResidentProver:
                     raise ValueError(f"blind: an array of shape ({N_BLIND}, 4) of raw Fr, True or False, not shape {scalars.shape}")
         return blinded, scalars
 
-    def _rounds(self, ch, blinded, scalars):
-        """rounds 1-5 from the wire and public-input evaluations in self.wire_eval / self.pub"""
+    def _rounds(self, challenges, blinded, scalars):
+        """rounds 1-5 from the wire and public-input evaluations in self.wire_eval / self.pub.  challenges(stage, outputs)
+        -> dict of raw Fr challenges, asked where the reference asks its transcript: "wires" (the 5 wire commitments) ->
+        beta, gamma; "perm" ([z's commitment]) -> alpha; "quot" (the 5 quotient-chunk commitments) -> zeta; "evals" (the
+        10 evaluations) -> v"""
         ctx, n, m, log_n, F = self.ctx, self.n, self.m, self.log_n, self.F
         log_m = log_n + 3
         com, P = [], lambda t: t.data_ptr()
@@ -239,12 +311,14 @@ class ResidentProver:
             if blinded:
                 ctx.poly_blind_dev(P(self.wire_coef[i]), n, BLIND_WIRE, None if scalars is None else scalars[BLIND_WIRE * i:BLIND_WIRE * (i + 1)])
             com.append(ctx.commit_dev(P(self.wire_coef[i]), nw))
+        ch = dict(challenges("wires", com[:N_WIRE]))
         # round 2
         ctx.perm_product_dev(P(self.wire_eval), P(self.id_eval), P(self.sig_eval), N_WIRE, n, ch["beta"], ch["gamma"], P(self.z))
         ctx.ntt_dev(P(self.z), log_n, True, False)
         if blinded:
             ctx.poly_blind_dev(P(self.z), n, BLIND_Z, None if scalars is None else scalars[N_WIRE * BLIND_WIRE:])
         com.append(ctx.commit_dev(P(self.z), nz))
+        ch.update(challenges("perm", com[N_WIRE:]))
         ctx.ntt_dev(P(self.pub), log_n, True, False)
         # round 3: 25 coset evaluations on the 8n domain, the quotient evaluations, one coset-iNTT(8n).  Blinded, the wires
         # and z are transformed on their first n coefficients and the quotient kernel adds the rest (their tails)
@@ -275,12 +349,14 @@ class ResidentProver:
         chunk = n + 2
         for j in range(N_WIRE):
             com.append(ctx.commit_dev(P(self.quot) + 32 * j * chunk, chunk))
+        ch.update(challenges("quot", com[N_WIRE + 1:]))
         # round 4
         zeta = ch["zeta"]
         zeta_w = F.mul(zeta, F.omega)
         w_ev = [ctx.poly_eval(P(self.wire_coef[i]), zeta, nw) for i in range(N_WIRE)]
         s_ev = [ctx.poly_eval(P(self.sig_coef[i]), zeta, n) for i in range(N_WIRE - 1)]
         z_next = ctx.poly_eval(P(self.z), zeta_w, nz)
+        ch.update(challenges("evals", w_ev + s_ev + [z_next]))
         # round 5: the scalar coefficients are host glue (a few dozen field operations), the polynomials stay put
         a, bb, c, d, e = w_ev
         ab, cd = F.mul(a, bb), F.mul(c, d)

@@ -3,7 +3,11 @@
 //!
 //!   cp rust/dump_fixtures.rs <reference>/src/bin/dump_fixtures.rs
 //!   (Cargo.toml: rand_chacha = "0.3" next to `rand`; nothing else)
-//!   cargo run --release --bin dump_fixtures -- ref_v1.bin && cp ref_v1.bin <this repo>/tests/golden/
+//!   cargo run --release --bin dump_fixtures -- ref_v1.bin ref_plonk_v1.bin && cp ref_v1.bin ref_plonk_v1.bin <this repo>/tests/golden/
+//!
+//! ref_plonk_v1.bin (same format) pins the Fiat-Shamir side: merlin 3.0.0 op sequences and the challenge bytes they give
+//! (TRANSCRIPT), and one small jf-plonk proof with its verifying key, public inputs, the six challenges jf-plonk's
+//! verifier derives, and the verify result (PLONK).  Consumer: tests/test_ref_plonk_fixture.py.
 //!
 //! Format: rust/README.md ("ref_v1.bin format").  Consumer: tests/test_ref_fixture.py (oracle on the CPU, the CUDA
 //! library with -m gpu), byte for byte.  NOT COMPILED in this repository (no Rust toolchain in the build image).
@@ -15,6 +19,11 @@ use ark_serialize::CanonicalSerialize;
 use hello_world::utils::serialize;
 use rand_chacha::{rand_core::SeedableRng, ChaCha20Rng};
 use std::{fs::File, io::Write};
+use ark_bls12_381::Bls12_381;
+use jf_plonk::prelude::*;
+use jf_plonk::proof_system::{PlonkKzgSnark, Snark};
+use jf_utils::to_bytes;
+use merlin::Transcript;
 
 const SEED: u64 = 0xD15791B07E5EED;
 
@@ -92,6 +101,126 @@ fn dist_fft(x: &[Fr], log: u32, is_inv: bool, is_coset: bool) -> Vec<Fr> {
         }
     }
     out
+}
+
+// ---- ref_plonk_v1.bin: the transcript and one jf-plonk proof
+const OP_NEW: u8 = 0;
+const OP_APPEND: u8 = 1;
+const OP_CHALLENGE: u8 = 2;
+
+/// one op of a TRANSCRIPT record: kind u8, label (u32 LE length + bytes), then the message (u32 LE length + bytes) of
+/// an append or the u32 LE byte count of a challenge
+fn op(ops: &mut Vec<u8>, kind: u8, label: &[u8], payload: &[u8]) {
+    ops.push(kind);
+    ops.extend_from_slice(&(label.len() as u32).to_le_bytes());
+    ops.extend_from_slice(label);
+    if kind == OP_APPEND {
+        ops.extend_from_slice(&(payload.len() as u32).to_le_bytes());
+    }
+    ops.extend_from_slice(payload);
+}
+
+fn transcript_record(o: &mut Out, msg_lens: &[usize], challenge_lens: &[usize]) {
+    let (mut ops, mut out, mut count) = (vec![], vec![], 0u64);
+    let mut t = Transcript::new(b"dump_fixtures");
+    op(&mut ops, OP_NEW, b"dump_fixtures", &[]);
+    count += 1;
+    for (i, &ln) in msg_lens.iter().enumerate() {
+        let m = (0..ln).map(|j| ((j * 7 + i) & 255) as u8).collect::<Vec<_>>();
+        t.append_message(b"m", &m);
+        op(&mut ops, OP_APPEND, b"m", &m);
+        let mut buf = vec![0u8; 64];
+        t.challenge_bytes(b"c", &mut buf);
+        op(&mut ops, OP_CHALLENGE, b"c", &64u32.to_le_bytes());
+        out.extend_from_slice(&buf);
+        count += 2;
+    }
+    for &k in challenge_lens {
+        let mut buf = vec![0u8; k];
+        t.challenge_bytes(b"k", &mut buf);
+        op(&mut ops, OP_CHALLENGE, b"k", &(k as u32).to_le_bytes());
+        out.extend_from_slice(&buf);
+        count += 1;
+    }
+    o.record(9, [count, 0, 0, 0], &[&ops, &out]);
+}
+
+/// get_and_append_challenge of dispatcher2.rs:144-153
+fn challenge(t: &mut Transcript, label: &'static [u8]) -> Fr {
+    let mut buf = [0u8; 64];
+    t.challenge_bytes(label, &mut buf);
+    let c = Fr::from_le_bytes_mod_order(&buf);
+    t.append_message(label, &to_bytes!(&c).unwrap());
+    c
+}
+
+fn plonk_record(o: &mut Out) {
+    let mut rng = o.rng();
+    let mut circuit = PlonkCircuit::<Fr>::new();
+    let x = circuit.create_public_variable(Fr::from(3u64)).unwrap();
+    let y = circuit.create_variable(Fr::from(4u64)).unwrap();
+    let s = circuit.add(x, y).unwrap();
+    let p = circuit.mul(s, y).unwrap();
+    let out = circuit.create_public_variable(Fr::from(28u64)).unwrap();
+    circuit.equal_gate(p, out).unwrap();
+    circuit.finalize_for_arithmetization().unwrap();
+    let srs = PlonkKzgSnark::<Bls12_381>::universal_setup(circuit.srs_size().unwrap(), &mut rng).unwrap();
+    let (pk, vk) = PlonkKzgSnark::<Bls12_381>::preprocess(&srs, &circuit).unwrap();
+    let proof = PlonkKzgSnark::<Bls12_381>::prove::<_, _, StandardTranscript>(&mut rng, &circuit, &pk).unwrap();
+    let pub_input = circuit.public_input().unwrap();
+    let ok = PlonkKzgSnark::<Bls12_381>::verify::<StandardTranscript>(&vk, &pub_input, &proof).is_ok();
+    // the verifier's transcript, as FakeStandardTranscript (dispatcher2.rs:44-154) and jf-plonk's verifier feed it
+    let mut t = Transcript::new(b"PlonkProof");
+    t.append_message(b"field size in bits", &Fr::size_in_bits().to_le_bytes());
+    t.append_message(b"domain size", &vk.domain_size.to_le_bytes());
+    t.append_message(b"input size", &vk.num_inputs.to_le_bytes());
+    let mut vk_bytes = vec![];
+    for k in vk.k.iter() {
+        vk_bytes.extend(to_bytes!(k).unwrap());
+        t.append_message(b"wire subsets separators", &to_bytes!(k).unwrap());
+    }
+    for c in vk.selector_comms.iter() {
+        vk_bytes.extend(to_bytes!(c).unwrap());
+        t.append_message(b"selector commitments", &to_bytes!(c).unwrap());
+    }
+    for c in vk.sigma_comms.iter() {
+        vk_bytes.extend(to_bytes!(c).unwrap());
+        t.append_message(b"sigma commitments", &to_bytes!(c).unwrap());
+    }
+    let mut pub_bytes = vec![];
+    for v in pub_input.iter() {
+        pub_bytes.extend(to_bytes!(v).unwrap());
+        t.append_message(b"public input", &to_bytes!(v).unwrap());
+    }
+    for c in proof.wires_poly_comms.iter() {
+        t.append_message(b"witness_poly_comms", &to_bytes!(c).unwrap());
+    }
+    let beta = challenge(&mut t, b"beta");
+    let gamma = challenge(&mut t, b"gamma");
+    t.append_message(b"perm_poly_comms", &to_bytes!(&proof.prod_perm_poly_comm).unwrap());
+    let alpha = challenge(&mut t, b"alpha");
+    for c in proof.split_quot_poly_comms.iter() {
+        t.append_message(b"quot_poly_comms", &to_bytes!(c).unwrap());
+    }
+    let zeta = challenge(&mut t, b"zeta");
+    for v in proof.poly_evals.wires_evals.iter() {
+        t.append_message(b"wire_evals", &to_bytes!(v).unwrap());
+    }
+    for v in proof.poly_evals.wire_sigma_evals.iter() {
+        t.append_message(b"wire_sigma_evals", &to_bytes!(v).unwrap());
+    }
+    t.append_message(b"perm_next_eval", &to_bytes!(&proof.poly_evals.perm_next_eval).unwrap());
+    let v = challenge(&mut t, b"v");
+    t.append_message(b"open_proof", &to_bytes!(&proof.opening_proof).unwrap());
+    t.append_message(b"shifted_open_proof", &to_bytes!(&proof.shifted_opening_proof).unwrap());
+    let u = challenge(&mut t, b"u");
+    let mut ch = vec![];
+    for c in [beta, gamma, alpha, zeta, v, u].iter() {
+        ch.extend(to_bytes!(c).unwrap());
+    }
+    let mut proof_bytes = vec![];
+    proof.serialize(&mut proof_bytes).unwrap();
+    o.record(10, [vk.domain_size as u64, vk.num_inputs as u64, 0, 0], &[&vk_bytes, &pub_bytes, &proof_bytes, &ch, &[ok as u8]]);
 }
 
 fn main() {
@@ -191,6 +320,17 @@ fn main() {
         }
         o.record(8, [pts.len() as u64, 0, 0, 0], &[serialize(&pts), &comp]);
     }
+    let n = o.count;
+    o.finish();
+    println!("{}: {} records", path, n);
+
+    // ref_plonk_v1.bin: 9 TRANSCRIPT, 10 PLONK
+    let path = std::env::args().nth(2).unwrap_or_else(|| "ref_plonk_v1.bin".to_string());
+    let mut o = Out { f: File::create(&path).unwrap(), count: 0, body: vec![] };
+    transcript_record(&mut o, &[0, 1, 32, 97], &[1, 32, 64]);
+    transcript_record(&mut o, &[165, 166, 167, 500], &[1, 2, 63, 64, 65, 165, 166, 167, 200]);
+    transcript_record(&mut o, &(0..170).collect::<Vec<_>>(), &[3]);
+    plonk_record(&mut o);
     let n = o.count;
     o.finish();
     println!("{}: {} records", path, n);

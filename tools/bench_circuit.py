@@ -5,6 +5,12 @@ n public-input evaluations in) on one prover.  Prints one JSON line.
 
     python tools/bench_circuit.py --log-n 22
     python tools/bench_circuit.py --log-n 24 --steps 2 --rounds 1
+    python tools/bench_circuit.py --log-n 22 --proof
+
+--proof: proofs a verifier accepts (prove_circuit, challenges from the transcript) instead of the prove_witness / prove
+alternation.  First prove_circuit with fixed blinders must equal prove_witness on the challenges it derived with the same
+blinders (13 commitments, 10 evaluations; exit code 3 otherwise), then prove_circuit and prove_witness (both blinded by
+the library) are timed alternately on one prover, with transcript_ms: the host time inside the transcript per proof.
 
 The circuit is bench_circuit_inputs' synthetic one: num_vars = 4n variables, slots on uniform random variables except the
 last n/8 gates, which all hold one padding variable.  Before anything is timed: the identity / sigma evaluations at 4096
@@ -93,11 +99,51 @@ def verify(ctx, torch, pr, vk, log_n, wire_vars, witness, ch):
     return out, (wires, pub)
 
 
+def proof_leg(torch, pr, witness, args, line) -> bool:
+    """--proof: the equality check, then prove_circuit and prove_witness alternately (both blinded by the library)"""
+    from distributed_plonk_b200.proof import Proof, fr_from_int
+    from distributed_plonk_b200.resident import N_BLIND
+    rng = np.random.default_rng(0xB11D)
+    fixed = np.stack([fr_from_int(int(rng.integers(1 << 62)) << 180 | int(rng.integers(1 << 62))) for _ in range(N_BLIND)])
+    proof, _ = pr.prove_circuit(witness, blind=fixed)
+    com, ev, _ = pr.prove_witness(witness, pr.last_challenges, blind=fixed)
+    ok = Proof.from_raw(com, ev) == proof
+    line["verify"]["prove_circuit_equals_prove_witness"] = bool(ok)
+    if not ok:
+        line["error"] = "prove_circuit and prove_witness on its challenges disagree"
+        return False
+    legs, tms = {"prove_circuit": [], "prove_witness": []}, []
+    ch = pr.last_challenges
+    for _ in range(args.rounds):
+        for name in legs:
+            fn = (lambda: pr.prove_circuit(witness)) if name == "prove_circuit" else (lambda: pr.prove_witness(witness, ch, blind=True))
+            fn()
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            for _ in range(args.steps):
+                fn()
+                if name == "prove_circuit":
+                    tms.append(pr.last_transcript_ms)
+            torch.cuda.synchronize()
+            legs[name].append(args.steps / (time.perf_counter() - t0))
+    for name, vals in legs.items():
+        line[name] = {"proofs_per_s": round(float(np.mean(vals)), 4), "values": [round(v, 4) for v in vals], "blind": True}
+    ms_per_proof = 1e3 / line["prove_circuit"]["proofs_per_s"]
+    line["transcript_ms"] = {"mean": round(float(np.mean(tms)), 3), "max": round(float(np.max(tms)), 3),
+                             "share_of_proof": round(float(np.mean(tms)) / ms_per_proof, 5),
+                             "what": "host time inside the transcript per prove_circuit: public inputs, 11 commitments converted "
+                                     "to affine and hashed, 10 evaluations, 5 challenges (the verifying-key prefix is hashed once, "
+                                     "by load_circuit), plus the proof object; host clock"}
+    line["proof_bytes"] = len(proof.to_bytes())
+    return True
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--log-n", type=int, default=22, dest="log_n")
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=2, help="alternations of prove_witness and prove")
+    ap.add_argument("--proof", action="store_true", help="time prove_circuit against prove_witness instead (module docstring)")
     args = ap.parse_args()
 
     import torch
@@ -144,7 +190,9 @@ def main():
                                 "what": "wire_permutation = sort + successor; perm_evals = identity and sigma evaluations; intt = 18 in-place "
                                         "iNTT(n); commit = the 18 verifying-key commitments (one MSM batch, or one per polynomial when round 3 is sliced); host clock, every step ends in a "
                                         "device synchronise; steps_ms is a second, warm call"}
-        legs = {"prove_witness": [], "prove": []}
+        legs = {} if args.proof else {"prove_witness": [], "prove": []}
+        if args.proof:
+            ok = proof_leg(torch, pr, witness, args, line)
         for _ in range(args.rounds):
             for name in legs:
                 fn = (lambda: pr.prove_witness(witness, ch)) if name == "prove_witness" else (lambda: pr.prove(wires, pub, ch))
@@ -158,17 +206,19 @@ def main():
                 legs[name].append(args.steps / (time.perf_counter() - t0))
         for name, vals in legs.items():
             line[name] = {"proofs_per_s": round(float(np.mean(vals)), 4), "values": [round(v, 4) for v in vals]}
-        line["prove_witness"]["h2d_bytes_per_proof"] = int(pr.num_vars * 32)
-        line["prove"]["h2d_bytes_per_proof"] = int((resident.N_WIRE + 1) * n * 32)
+        if not args.proof:
+            line["prove_witness"]["h2d_bytes_per_proof"] = int(pr.num_vars * 32)
+            line["prove"]["h2d_bytes_per_proof"] = int((resident.N_WIRE + 1) * n * 32)
         free1, _ = torch.cuda.mem_get_info()
         torch_peak, torch_now = torch.cuda.max_memory_reserved(), torch.cuda.memory_reserved()
         line["device_memory"] = {"peak_gib_bound": round(((total - free1) - torch_now + torch_peak) / 2**30, 3),
                                  "in_use_before_gib": round((total - free0) / 2**30, 3), "device_total_gib": round(total / 2**30, 3),
                                  "how": "device memory in use at the end (the library's pool keeps its peak), minus torch's reserve now, "
                                         "plus torch's peak reserve since the prover was built (an upper bound of the peak)"}
-        line["value"] = line["prove_witness"]["proofs_per_s"]
-    else:
-        line["error"] = "the preprocessing or the proof from the witness disagrees with its check"
+        if ok:
+            line["value"] = line["prove_circuit" if args.proof else "prove_witness"]["proofs_per_s"]
+    if not ok:
+        line.setdefault("error", "the preprocessing or the proof from the witness disagrees with its check")
     print(json.dumps(line), flush=True)
     ctx.close()
     if not ok:
