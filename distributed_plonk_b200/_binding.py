@@ -21,6 +21,7 @@ EXPORTS = [
     "dp_ntt_dev_quot_slice", "dp_quotient_evals_slice_dev",
     "dp_poly_blind_dev", "dp_quotient_evals_tail_dev", "dp_quotient_evals_slice_tail_dev",
     "dp_wire_permutation_scratch_bytes", "dp_wire_permutation_dev", "dp_perm_evals_dev", "dp_witness_gather_dev", "dp_commit_dev_batch",
+    "dp_srs_powers_of_tau",
 ]
 
 
@@ -116,6 +117,7 @@ def bind(cdll: C.CDLL) -> C.CDLL:
         "dp_perm_evals_dev": (i, [vp, vp, sz, sz, vp, vp, vp]),
         "dp_witness_gather_dev": (i, [vp, vp, u64, vp, sz, sz, sz, vp, vp]),
         "dp_commit_dev_batch": (i, [vp, sz, C.POINTER(vp), C.POINTER(sz), vp]),
+        "dp_srs_powers_of_tau": (i, [vp, vp, sz, vp]),
         "dp_poly_eval": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_eval_dev": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_lincomb": (i, [vp, C.POINTER(vp), C.POINTER(sz), vp, sz, vp, sz]),
@@ -559,6 +561,22 @@ class Context:
     def gen_bases_into(self, seed: int, n: int, out_ptr: int):
         """the same, written to `out_ptr` (n * 104 B of host or device memory)"""
         self._ck(self.lib.dp_debug_gen_bases(self.h, seed, n, out_ptr))
+
+    @staticmethod
+    def _tau_bytes(tau: int) -> bytes:
+        if not 0 <= int(tau) < 1 << 256:
+            raise ValueError("tau must be an integer in [0, 2^256); the library accepts 0 < tau < r")
+        return int(tau).to_bytes(32, "little")
+
+    def srs_powers_of_tau(self, tau: int, n: int) -> np.ndarray:
+        """[n, 104] raw G1Affine: row i = tau^i * G1 (tau a canonical integer, 0 < tau < r)"""
+        out = np.zeros((n, G1_AFFINE_BYTES), dtype=np.uint8)
+        self._ck(self.lib.dp_srs_powers_of_tau(self.h, self._tau_bytes(tau), n, _addr(out) if n else None))
+        return out
+
+    def srs_powers_of_tau_into(self, tau: int, n: int, out_ptr: int):
+        """the same, written to `out_ptr` (n * 104 B of host or device memory)"""
+        self._ck(self.lib.dp_srs_powers_of_tau(self.h, self._tau_bytes(tau), n, out_ptr))
 
     def init_ptr(self, bases_ptr: int, n_bases: int, domain_size: int, quot_domain_size: int):
         """PlonkSlave.init with the raw GroupAffine array at `bases_ptr` (host or device memory)"""

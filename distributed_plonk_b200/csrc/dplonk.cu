@@ -19,6 +19,7 @@
 #include "ntt.cuh"
 #include "perm.cuh"
 #include "rounds.cuh"
+#include "srs.cuh"
 
 using namespace dp;
 
@@ -198,6 +199,8 @@ struct dp_ctx {
     // first dp_quotient_evals after dp_init when it fits (32 B per point), dropped by the next dp_init
     Fr *quot_inv = nullptr;
     uint32_t quot_inv_log = 0;
+    // fixed-base table of dp_srs_powers_of_tau (srs.cuh, 48 MiB): built by its first call, dropped by the next dp_init
+    G1Affine *srs_table = nullptr;
     // batched-affine tree levels in front of the XYZZ chunks (msm.cuh): 0 = none, else L.  env DP_MSM_AFFINE=L forces L levels;
     // otherwise dp_init chooses by msm_tune() - one MSM over the context's own window table per candidate, results compared
     // byte for byte, levels kept only if identical and faster (an SRS whose hot-path MSM has fewer than msm_affine_min_digits
@@ -1531,6 +1534,8 @@ static int init_impl(dp_ctx *ctx, const void *bases, size_t n_bases, uint64_t do
     free_domain(ctx, ctx->dom[1]);
     ctx->pool.release(ctx->quot_inv);
     ctx->quot_inv = nullptr;
+    ctx->pool.release(ctx->srs_table);
+    ctx->srs_table = nullptr;
     ctx->inited = false;
     ctx->n_bases = n_bases;
     if (n_bases) {
@@ -2642,6 +2647,87 @@ int dp_debug_gen_bases(dp_ctx *ctx, uint64_t seed, size_t n, void *out) {
     ctx->pool.release(dev);
     if (e != cudaSuccess) return fail(ctx, DP_E_CUDA, "dp_debug_gen_bases: %s", cudaGetErrorString(e));
     return DP_OK;
+}
+
+int dp_srs_powers_of_tau(dp_ctx *ctx, const void *tau32, size_t n, void *out104) {
+    if (!ctx) return fail(ctx, DP_E_ARG, "dp_srs_powers_of_tau: ctx is NULL");
+    if (n && (!tau32 || !out104)) return fail(ctx, DP_E_ARG, "dp_srs_powers_of_tau: NULL argument");
+    if (n == 0) return DP_OK;
+    if (n > ((uint64_t)1 << 32)) return fail(ctx, DP_E_ARG, "dp_srs_powers_of_tau: %zu points exceed 2^32", n);
+    Fr tau;
+    memcpy(tau.l, tau32, sizeof tau.l);
+    if (tau.is_zero()) return fail(ctx, DP_E_ARG, "dp_srs_powers_of_tau: tau is zero");
+    if (!tau.canon_is_reduced()) return fail(ctx, DP_E_ARG, "dp_srs_powers_of_tau: tau is not a canonical scalar (tau >= r)");
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    // tau^i = A[i mod 2^h] * B[i >> h]: A[a] = tau^a, B[b] = tau^(2^h b), about sqrt(n) host products each
+    const uint32_t log_a = (log2_ceil_u64(n) + 1) / 2;
+    const uint64_t n_a = (uint64_t)1 << log_a, n_b = (n + n_a - 1) >> log_a;
+    std::vector<Fr> pow_a(n_a), pow_b(n_b);
+    const Fr t = tau.to_mont();
+    pow_a[0] = Fr::one();
+    for (uint64_t a = 1; a < n_a; a++) pow_a[a] = pow_a[a - 1] * t;
+    const Fr step = pow_a[n_a - 1] * t;
+    pow_b[0] = Fr::one();
+    for (uint64_t b = 1; b < n_b; b++) pow_b[b] = pow_b[b - 1] * step;
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    Fr *da = tmp.get<Fr>(n_a), *db = tmp.get<Fr>(n_b);
+    const uint64_t chunk = n < SRS_CHUNK ? n : SRS_CHUNK;
+    uint64_t *staging = tmp.get<uint64_t>(chunk * 13);
+    if (!da || !db || !staging) return fail(ctx, DP_E_OOM, "dp_srs_powers_of_tau buffers");
+    DP_CUDA(ctx, cudaMemcpyAsync(da, pow_a.data(), n_a * sizeof(Fr), cudaMemcpyHostToDevice, ctx->stream));
+    DP_CUDA(ctx, cudaMemcpyAsync(db, pow_b.data(), n_b * sizeof(Fr), cudaMemcpyHostToDevice, ctx->stream));
+    G1Affine *table = ctx->srs_table;
+    const bool build_table = !table;
+    std::vector<G1Affine> half_base;
+    if (build_table) {
+        // P_q = 2^(q c / 2) G, q < 2 * windows: the points whose small multiples build the fixed-base table
+        half_base.resize(2 * SRS_WINDOWS);
+        G1XYZZ p = G1XYZZ::from_affine(g1_generator());
+        for (uint32_t q = 0; q < 2 * SRS_WINDOWS; q++) {
+            if (q)
+                for (uint32_t k = 0; k < SRS_HALF; k++) p = p.dbl();
+            half_base[q] = p.to_affine(true);
+        }
+        G1Affine *dbase = tmp.get<G1Affine>(2 * SRS_WINDOWS), *mult = tmp.get<G1Affine>(SRS_MULTIPLES);
+        table = (G1Affine *)ctx->pool.alloc((size_t)SRS_WINDOWS * SRS_ROW * sizeof(G1Affine));
+        if (!dbase || !mult || !table) {
+            ctx->pool.release(table);
+            return fail(ctx, DP_E_OOM, "dp_srs_powers_of_tau table");
+        }
+        const cudaError_t e = cudaMemcpyAsync(dbase, half_base.data(), 2 * SRS_WINDOWS * sizeof(G1Affine), cudaMemcpyHostToDevice, ctx->stream);
+        if (e != cudaSuccess) {
+            ctx->pool.release(table);
+            return fail(ctx, DP_E_CUDA, "dp_srs_powers_of_tau: %s", cudaGetErrorString(e));
+        }
+        DP_LAUNCH(srs_multiples_kernel, dim3(blocks_for(SRS_MULTIPLES, AFF_TPB)), dim3(AFF_TPB), 0, ctx->stream, (const G1Affine *)dbase, mult);
+        DP_LAUNCH(srs_table_kernel, dim3(blocks_for(SRS_WINDOWS * SRS_ROW / SRS_TABLE_GROUP, 128)), dim3(128), 0, ctx->stream,
+                  (const G1Affine *)mult, table);
+        ctx->launches += 2;
+    }
+    const MsmGeom g = msm_make_geom(SRS_C, true, 0);
+    int rc = DP_OK;
+    for (uint64_t first = 0; first < n && rc == DP_OK; first += chunk) {
+        const uint64_t end = first + chunk < n ? first + chunk : n;
+        DP_LAUNCH(srs_powers_kernel, dim3(blocks_for(end - first, AFF_TPB)), dim3(AFF_TPB), 0, ctx->stream, (const Fr *)da,
+                  (const Fr *)db, log_a, first, end, g, (const G1Affine *)table, staging);
+        ctx->launches++;
+        cudaError_t e = cudaGetLastError();
+        if (e == cudaSuccess)
+            e = cudaMemcpyAsync((uint8_t *)out104 + first * DP_G1_AFFINE_BYTES, staging, (end - first) * DP_G1_AFFINE_BYTES, cudaMemcpyDefault,
+                                ctx->stream);  // host or device memory
+        if (e != cudaSuccess) rc = fail(ctx, DP_E_CUDA, "dp_srs_powers_of_tau: %s", cudaGetErrorString(e));
+    }
+    if (rc == DP_OK) rc = call_end(ctx, true);
+    if (build_table) {  // kept for the next call only when its build is known to have completed
+        if (rc == DP_OK) {
+            ctx->srs_table = table;
+        } else {
+            cudaStreamSynchronize(ctx->stream);
+            ctx->pool.release(table);
+        }
+    }
+    return rc;
 }
 
 int dp_debug_set_limits(dp_ctx *ctx, uint32_t max_contig_log_k, uint32_t max_strided_log_k, int msm_window_bits) {

@@ -79,6 +79,14 @@ int dp_init_compressed(dp_ctx *ctx, const void *bases48, size_t n_bases, uint64_
 /* bases [start, start + n) back as raw G1Affine (104 B each; identity = (0, 1, true))             */
 int dp_get_bases(dp_ctx *ctx, uint64_t start, size_t n, void *out104);
 
+/* KZG powers of tau for a test setup (jf-plonk PlonkKzgSnark::universal_setup, dispatcher2.rs:1279):
+ * out104[i] = tau^i * G1 for i < n, raw G1Affine (104 B, the layout dp_init reads).  tau32: 32 B canonical,
+ * 0 < tau < r, else DP_E_ARG.  out104: host memory or device memory of the context's GPU.  Needs no dp_init
+ * and leaves an initialised context's state as it was; its first call builds a 48 MiB fixed-base table that
+ * the context keeps until the next dp_init.  Returns when the points are written.  n = 0 writes nothing;
+ * n > 2^32 is DP_E_ARG.  Whoever knows tau can forge proofs against this SRS.                             */
+int dp_srs_powers_of_tau(dp_ctx *ctx, const void *tau32, size_t n, void *out104);
+
 /* ---- PlonkSlave.varMsm (src/worker.rs:159-185) -----------------------------------------------
  * out = sum_{k < min(end-start, n_scalars)} scalars[k] * bases[start + k]
  * (VariableBaseMSM::multi_scalar_mul(&bases[start..end], &scalars) truncates to the shorter).
