@@ -194,6 +194,10 @@ struct dp_ctx {
     int ntt_min_blocks = 3;    // knob (env DP_NTT_BLOCKS): register budget of ntt_tile_kernel for 2 or 3 CTAs per SM (3: -7 % per transform)
     uint32_t msm_chunk = 0;    // experiment knob (env DP_MSM_CHUNK): digits per accumulate thread, 0 = default
     int msm_force_c = 0;       // 0 auto, 1 = windowed path with automatic c, >= 2 forced c (windowed)
+    // knob (env DP_MSM_PRE_C): width of the window-multiple table built by dp_init.  Unset = msm_pick_pre_c's choice within
+    // a quarter of the free memory; 0 = no table (pre_disabled: every MSM takes the per-window pipeline); 8..22 = exactly
+    // that width or dp_init fails (DP_E_ARG when the width cannot index the shard, DP_E_OOM when the table does not fit)
+    int msm_pre_c = -1;        // -1 = unset; a value that does not parse is kept as out of range and refused by dp_init
     bool pre_disabled = false;
     // 1 / (x_i - 1) over the quotient coset (rounds.cuh: quotient_kernel<true>): depends on the domain only, built by the
     // first dp_quotient_evals after dp_init when it fits (32 B per point), dropped by the next dp_init
@@ -1412,6 +1416,12 @@ int dp_create(int cuda_device, uint64_t me, uint64_t n_workers, dp_ctx **out) {
     }
     if (const char *e = getenv("DP_MSM_AFFINE_MIN")) ctx->msm_affine_min_digits = strtoull(e, nullptr, 10);
     if (const char *e = getenv("DP_MSM_TUNE")) ctx->msm_tune_mode = atoi(e) < 0 ? 0 : atoi(e) > 2 ? 2 : atoi(e);
+    if (const char *e = getenv("DP_MSM_PRE_C")) {
+        char *end = nullptr;
+        const long v = strtol(e, &end, 10);
+        ctx->msm_pre_c = end != e && *end == '\0' && v >= 0 && v <= 64 ? (int)v : 1000;
+        ctx->pre_disabled = ctx->msm_pre_c == 0;
+    }
     ctx->me = me;
     ctx->W = n_workers;
     int rc = DP_OK;
@@ -1511,6 +1521,8 @@ static int init_impl(dp_ctx *ctx, const void *bases, size_t n_bases, uint64_t do
     if (!ctx) return DP_E_ARG;
     if (n_bases && !bases) return fail(ctx, DP_E_ARG, "dp_init: bases is NULL");
     if (domain_size == 0 || quot_domain_size == 0) return fail(ctx, DP_E_ARG, "dp_init: domain sizes must be >= 1");
+    if (ctx->msm_pre_c > 0 && (ctx->msm_pre_c < 8 || ctx->msm_pre_c > 22))
+        return fail(ctx, DP_E_ARG, "dp_init: DP_MSM_PRE_C must be 0 or a table width of 8 to 22");
     DP_CUDA(ctx, cudaSetDevice(ctx->device));
     call_begin(ctx);
     // drop previous state (init may be called again, worker.rs:135-141 overwrites)
@@ -1570,10 +1582,20 @@ static int init_impl(dp_ctx *ctx, const void *bases, size_t n_bases, uint64_t do
         size_t free_b = 0, total_b = 0;
         cudaMemGetInfo(&free_b, &total_b);
         const uint64_t lo = ctx->me * n_bases / ctx->W, hi = (ctx->me + 1) * n_bases / ctx->W, span = hi - lo;
-        const uint32_t c = span >= (1u << 11) && !ctx->pre_disabled ? msm_pick_pre_c(span, free_b / 4) : 0;
+        uint32_t c = span >= (1u << 11) && !ctx->pre_disabled ? msm_pick_pre_c(span, free_b / 4) : 0;
+        if (ctx->msm_pre_c > 0) {  // pinned width: exactly this table or an error, never another width
+            c = (uint32_t)ctx->msm_pre_c;
+            const uint64_t nw = (256 + c - 1) / c;
+            if (span < (1u << 11) || nw * span >= (1ull << 31))
+                return fail(ctx, DP_E_ARG, "dp_init: DP_MSM_PRE_C=%u does not fit a shard of %llu bases (needs >= 2^11 and %llu windows * bases < 2^31)",
+                            c, (unsigned long long)span, (unsigned long long)nw);
+        }
         if (c) {
             const uint32_t nw = (256 + c - 1) / c;
             ctx->pre_table = nw <= (uint32_t)MSM_PRE_MAX_WINDOWS ? (G1Affine *)ctx->pool.alloc((size_t)nw * span * sizeof(G1Affine)) : nullptr;
+            if (!ctx->pre_table && ctx->msm_pre_c > 0)
+                return fail(ctx, DP_E_OOM, "dp_init: DP_MSM_PRE_C=%u: no room for the %.1f GB window table of %llu bases", c,
+                            (double)nw * span * sizeof(G1Affine) / 1e9, (unsigned long long)span);
             if (ctx->pre_table) {
                 ctx->pre_c = c;
                 ctx->pre_nw = nw;
