@@ -7,6 +7,7 @@ import numpy as np
 
 DP_OK, DP_E_ARG, DP_E_STATE, DP_E_OOM, DP_E_CUDA, DP_E_COMM = 0, -1, -2, -3, -4, -5
 FR_BYTES, G1_AFFINE_BYTES, G1_PROJECTIVE_BYTES = 32, 104, 144
+G1_COMPRESSED_BYTES, G2_AFFINE_BYTES, FQ12_BYTES = 48, 200, 576
 
 EXPORTS = [
     "dp_create", "dp_destroy", "dp_last_error", "dp_version", "dp_init", "dp_msm", "dp_commit", "dp_fft_init",
@@ -22,6 +23,7 @@ EXPORTS = [
     "dp_poly_blind_dev", "dp_quotient_evals_tail_dev", "dp_quotient_evals_slice_tail_dev",
     "dp_wire_permutation_scratch_bytes", "dp_wire_permutation_dev", "dp_perm_evals_dev", "dp_witness_gather_dev", "dp_commit_dev_batch",
     "dp_srs_powers_of_tau",
+    "dp_g1_decompress", "dp_msm_points", "dp_srs_open_key", "dp_multi_pairing",
 ]
 
 
@@ -29,6 +31,7 @@ class DpError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"dplonk error {code}: {msg}")
         self.code = code
+        self.msg = msg
 
 
 class FftWorkload(C.Structure):
@@ -118,6 +121,10 @@ def bind(cdll: C.CDLL) -> C.CDLL:
         "dp_witness_gather_dev": (i, [vp, vp, u64, vp, sz, sz, sz, vp, vp]),
         "dp_commit_dev_batch": (i, [vp, sz, C.POINTER(vp), C.POINTER(sz), vp]),
         "dp_srs_powers_of_tau": (i, [vp, vp, sz, vp]),
+        "dp_g1_decompress": (i, [vp, vp, sz, i, vp, C.POINTER(sz), C.POINTER(i)]),
+        "dp_msm_points": (i, [vp, vp, vp, sz, vp]),
+        "dp_srs_open_key": (i, [vp, vp, vp]),
+        "dp_multi_pairing": (i, [vp, vp, vp, sz, vp]),
         "dp_poly_eval": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_eval_dev": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_lincomb": (i, [vp, C.POINTER(vp), C.POINTER(sz), vp, sz, vp, sz]),
@@ -577,6 +584,50 @@ class Context:
     def srs_powers_of_tau_into(self, tau: int, n: int, out_ptr: int):
         """the same, written to `out_ptr` (n * 104 B of host or device memory)"""
         self._ck(self.lib.dp_srs_powers_of_tau(self.h, self._tau_bytes(tau), n, out_ptr))
+
+    # ---- verifier (none of these needs init)
+    def g1_decompress(self, points48, check_subgroup: bool = True) -> np.ndarray:
+        """[n, 48] ark-serialize compressed points -> [n, 104] raw G1Affine.  A rejected point raises DpError with
+        `index` (the first bad point) and `why` (1 x >= p, 2 both flags, 3 no such point, 4 outside the subgroup)"""
+        b = np.ascontiguousarray(points48, dtype=np.uint8).reshape(-1, G1_COMPRESSED_BYTES)
+        n = b.shape[0]
+        out = np.zeros((n, G1_AFFINE_BYTES), dtype=np.uint8)
+        idx, why = C.c_size_t(), C.c_int()
+        rc = self.lib.dp_g1_decompress(self.h, _addr(b) if n else None, n, int(check_subgroup), _addr(out) if n else None,
+                                       C.byref(idx), C.byref(why))
+        if rc != DP_OK:
+            err = DpError(rc, (self.lib.dp_last_error(self.h) or b"").decode())
+            err.index, err.why = idx.value, why.value
+            raise err
+        return out
+
+    def msm_points(self, points104, scalars) -> np.ndarray:
+        """sum scalars[i] * points[i]: [n, 104] raw G1Affine, [n, 4] u64 canonical scalars -> 144 B normalised Jacobian"""
+        pts = np.ascontiguousarray(points104, dtype=np.uint8).reshape(-1, G1_AFFINE_BYTES)
+        sc = np.ascontiguousarray(scalars, dtype=np.uint64).reshape(-1, 4)
+        if pts.shape[0] != sc.shape[0]:
+            raise ValueError(f"{pts.shape[0]} points but {sc.shape[0]} scalars")
+        n = pts.shape[0]
+        out = np.zeros(G1_PROJECTIVE_BYTES, dtype=np.uint8)
+        self._ck(self.lib.dp_msm_points(self.h, _addr(pts) if n else None, _addr(sc) if n else None, n, _addr(out)))
+        return out
+
+    def srs_open_key(self, tau: int) -> np.ndarray:
+        """[2, 200] raw G2Affine: H and tau * H (tau a canonical integer, 0 < tau < r)"""
+        out = np.zeros((2, G2_AFFINE_BYTES), dtype=np.uint8)
+        self._ck(self.lib.dp_srs_open_key(self.h, self._tau_bytes(tau), _addr(out)))
+        return out
+
+    def multi_pairing(self, g1_104, g2_200) -> np.ndarray:
+        """prod e(P_i, Q_i) over [k, 104] raw G1Affine and [k, 200] raw G2Affine -> 576 B Fq12 (12 Montgomery Fq)"""
+        p = np.ascontiguousarray(g1_104, dtype=np.uint8).reshape(-1, G1_AFFINE_BYTES)
+        q = np.ascontiguousarray(g2_200, dtype=np.uint8).reshape(-1, G2_AFFINE_BYTES)
+        if p.shape[0] != q.shape[0]:
+            raise ValueError(f"{p.shape[0]} G1 points but {q.shape[0]} G2 points")
+        k = p.shape[0]
+        out = np.zeros(FQ12_BYTES, dtype=np.uint8)
+        self._ck(self.lib.dp_multi_pairing(self.h, _addr(p) if k else None, _addr(q) if k else None, k, _addr(out)))
+        return out
 
     def init_ptr(self, bases_ptr: int, n_bases: int, domain_size: int, quot_domain_size: int):
         """PlonkSlave.init with the raw GroupAffine array at `bases_ptr` (host or device memory)"""

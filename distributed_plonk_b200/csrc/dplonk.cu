@@ -19,6 +19,7 @@
 #include "ntt.cuh"
 #include "perm.cuh"
 #include "rounds.cuh"
+#include "pairing.cuh"
 #include "srs.cuh"
 
 using namespace dp;
@@ -949,8 +950,10 @@ struct MsmPending {
 // `ready`: an event after which the scalars are complete AND every earlier user of the pool blocks this job may be
 // handed has finished (a batch records one on the compute stream before it queues anything, so that the sorts of all
 // its jobs can run ahead); nullptr = the compute stream as it stands now.
+// `points`: the bases are these n device points (dp_msm_points) instead of the context's SRS from `start` on; such an MSM
+// always takes the per-window pipeline (no window-multiple table exists for them).
 int msm_enqueue(dp_ctx *ctx, uint64_t start, const uint4 *scalars_dev, uint64_t n, G1JacobianOut *out_dev, MsmJob &job,
-                bool record_breakdown, cudaEvent_t ready = nullptr) {
+                bool record_breakdown, cudaEvent_t ready = nullptr, const G1Affine *points = nullptr) {
     cudaStream_t st = ctx->stream, tl = ctx->s_tail, so = ctx->msm_sort_own_stream ? ctx->s_sort : ctx->stream;
     if (n == 0) {
         static const G1JacobianOut id = G1JacobianOut::from_affine(G1Affine::inf());
@@ -959,12 +962,12 @@ int msm_enqueue(dp_ctx *ctx, uint64_t start, const uint4 *scalars_dev, uint64_t 
     }
     if (n >= ((uint64_t)1 << 31)) return fail(ctx, DP_E_ARG, "msm: %llu points exceed 2^31", (unsigned long long)n);
     // precomputed window multiples pay off once the shared bucket set is reasonably filled
-    const bool use_pre = ctx->pre_table && ctx->msm_force_c == 0 && start >= ctx->pre_lo && start + n <= ctx->pre_hi &&
+    const bool use_pre = !points && ctx->pre_table && ctx->msm_force_c == 0 && start >= ctx->pre_lo && start + n <= ctx->pre_hi &&
                          n * ctx->pre_nw >= 4ull * (1ull << (ctx->pre_c - 1));
     MsmGeom g = use_pre ? msm_make_geom(ctx->pre_c, true, ctx->pre_hi - ctx->pre_lo)
                         : msm_geometry(n, ctx->msm_force_c > 1 ? ctx->msm_force_c : 0);
     if (ctx->msm_chunk) g.chunk = ctx->msm_chunk;
-    const G1Affine *bases = use_pre ? ctx->pre_table + (start - ctx->pre_lo) : ctx->bases + start;
+    const G1Affine *bases = points ? points : use_pre ? ctx->pre_table + (start - ctx->pre_lo) : ctx->bases + start;
     const uint64_t max_digits = n * g.n_windows;
     // L batched-affine tree levels in front of the XYZZ chunks (msm.cuh): every bucket's slice of the sorted array is padded
     // to a multiple of 2^L entries, the chunk kernel then sees 1 / 2^L of the entries
@@ -1113,10 +1116,10 @@ int msm_finish(dp_ctx *ctx, std::vector<MsmJob> &jobs, bool breakdown) {
 }
 
 int msm_device(dp_ctx *ctx, uint64_t start, const uint4 *scalars_dev, uint64_t n, G1JacobianOut *out_dev,
-               uint32_t *err_host_out) {
+               uint32_t *err_host_out, const G1Affine *points = nullptr) {
     (void)err_host_out;
     std::vector<MsmJob> jobs(1);
-    int rc = msm_enqueue(ctx, start, scalars_dev, n, out_dev, jobs[0], n != 0);
+    int rc = msm_enqueue(ctx, start, scalars_dev, n, out_dev, jobs[0], n != 0, nullptr, points);
     int rc2 = msm_finish(ctx, jobs, rc == DP_OK && n != 0);
     return rc != DP_OK ? rc : rc2;
 }
@@ -1514,6 +1517,10 @@ int dp_last_timing(const dp_ctx *ctx, float *kernel_ms, uint64_t *launches) {
 
 uint64_t dp_launch_count(const dp_ctx *ctx) { return ctx ? ctx->launches : 0; }
 
+// g1_decompress_kernel's reason codes (msm.cuh)
+static const char *const G1_DECOMPRESS_WHY[] = {"", "x is not a canonical field element", "both flag bits set",
+                                                "x^3 + 4 is not a square: no such point", "the point is not in the r-torsion subgroup"};
+
 // format 0: raw ark GroupAffine structs (104 B, utils.rs:27-43) - what the reference's init RPC carries;
 // format 1: ark-serialize compressed points (48 B) - what SRS files hold ("next" row 4)
 static int init_impl(dp_ctx *ctx, const void *bases, size_t n_bases, uint64_t domain_size, uint64_t quot_domain_size, int format,
@@ -1569,12 +1576,11 @@ static int init_impl(dp_ctx *ctx, const void *bases, size_t n_bases, uint64_t do
             DP_CUDA(ctx, cudaMemcpyAsync(&verdict, err, sizeof verdict, cudaMemcpyDeviceToHost, ctx->stream));
             DP_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
             if (verdict != ~0ull) {
-                static const char *why[] = {"", "x is not a canonical field element", "both flag bits set", "x^3 + 4 is not a square: no such point",
-                                            "the point is not in the r-torsion subgroup"};
                 ctx->pool.release(ctx->bases);
                 ctx->bases = nullptr;
                 ctx->n_bases = 0;
-                return fail(ctx, DP_E_ARG, "dp_init_compressed: point %llu rejected: %s", (unsigned long long)((verdict >> 8) - 1), why[verdict & 7]);
+                return fail(ctx, DP_E_ARG, "dp_init_compressed: point %llu rejected: %s", (unsigned long long)((verdict >> 8) - 1),
+                            G1_DECOMPRESS_WHY[verdict & 7]);
             }
         }
         ctx->launches++;
@@ -2750,6 +2756,114 @@ int dp_srs_powers_of_tau(dp_ctx *ctx, const void *tau32, size_t n, void *out104)
         }
     }
     return rc;
+}
+
+// ---- verifier: decoding, an MSM over caller-given points, the G2 open key and the multi-pairing (pairing.cuh)
+int dp_g1_decompress(dp_ctx *ctx, const void *in48, size_t n, int check_subgroup, void *out104, size_t *bad_index, int *why) {
+    if (!ctx) return fail(ctx, DP_E_ARG, "dp_g1_decompress: ctx is NULL");
+    if (n && (!in48 || !out104)) return fail(ctx, DP_E_ARG, "dp_g1_decompress: NULL argument");
+    if (bad_index) *bad_index = n;
+    if (why) *why = 0;
+    if (n == 0) return DP_OK;
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    uint32_t *staging = tmp.get<uint32_t>(n * 12);
+    G1Affine *pts = tmp.get<G1Affine>(n);
+    uint64_t *raw = tmp.get<uint64_t>(n * 13);
+    unsigned long long *err = tmp.get<unsigned long long>(1), verdict = ~0ull;
+    if (!staging || !pts || !raw || !err) return fail(ctx, DP_E_OOM, "dp_g1_decompress buffers");
+    DP_CUDA(ctx, cudaMemcpyAsync(staging, in48, n * (size_t)DP_G1_COMPRESSED_BYTES, cudaMemcpyHostToDevice, ctx->stream));
+    DP_CUDA(ctx, cudaMemcpyAsync(err, &verdict, sizeof verdict, cudaMemcpyHostToDevice, ctx->stream));
+    DP_LAUNCH(g1_decompress_kernel, dim3(blocks_for(n, 128)), dim3(128), 0, ctx->stream, (const uint32_t *)staging, pts, (uint64_t)n,
+              check_subgroup ? 1u : 0u, err);
+    DP_LAUNCH(g1_export_ark_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, ctx->stream, (const G1Affine *)pts, raw, (uint64_t)n);
+    ctx->launches += 2;
+    DP_CUDA(ctx, cudaMemcpyAsync(&verdict, err, sizeof verdict, cudaMemcpyDeviceToHost, ctx->stream));
+    DP_TRY(call_end(ctx, true));
+    if (verdict != ~0ull) {
+        const size_t idx = (size_t)((verdict >> 8) - 1);
+        if (bad_index) *bad_index = idx;
+        if (why) *why = (int)(verdict & 7);
+        return fail(ctx, DP_E_ARG, "dp_g1_decompress: point %zu rejected: %s", idx, G1_DECOMPRESS_WHY[verdict & 7]);
+    }
+    DP_CUDA(ctx, cudaMemcpy(out104, raw, n * (size_t)DP_G1_AFFINE_BYTES, cudaMemcpyDeviceToHost));
+    return DP_OK;
+}
+
+int dp_msm_points(dp_ctx *ctx, const void *points104, const void *scalars32, size_t n, void *out144) {
+    if (!ctx) return fail(ctx, DP_E_ARG, "dp_msm_points: ctx is NULL");
+    if (!out144 || (n && (!points104 || !scalars32))) return fail(ctx, DP_E_ARG, "dp_msm_points: NULL argument");
+    if (n >= ((uint64_t)1 << 31)) return fail(ctx, DP_E_ARG, "dp_msm_points: %zu points exceed 2^31", n);
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    uint64_t *raw = tmp.get<uint64_t>(n * 13);
+    G1Affine *pts = tmp.get<G1Affine>(n);
+    uint4 *sc = tmp.get<uint4>(2 * n);
+    G1JacobianOut *od = tmp.get<G1JacobianOut>(1);
+    if (!raw || !pts || !sc || !od) return fail(ctx, DP_E_OOM, "dp_msm_points buffers for %zu points", n);
+    if (n) {
+        DP_CUDA(ctx, cudaMemcpyAsync(raw, points104, n * (size_t)DP_G1_AFFINE_BYTES, cudaMemcpyHostToDevice, ctx->stream));
+        DP_CUDA(ctx, cudaMemcpyAsync(sc, scalars32, n * 32, cudaMemcpyHostToDevice, ctx->stream));
+        DP_LAUNCH(g1_import_ark_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, ctx->stream, (const uint64_t *)raw, pts, (uint64_t)n);
+        ctx->launches++;
+    }
+    DP_TRY(msm_device(ctx, 0, sc, n, od, nullptr, pts));
+    DP_CUDA(ctx, cudaMemcpyAsync(out144, od, sizeof(G1JacobianOut), cudaMemcpyDeviceToHost, ctx->stream));
+    return call_end(ctx, true);
+}
+
+int dp_srs_open_key(dp_ctx *ctx, const void *tau32, void *out400) {
+    if (!ctx) return fail(ctx, DP_E_ARG, "dp_srs_open_key: ctx is NULL");
+    if (!tau32 || !out400) return fail(ctx, DP_E_ARG, "dp_srs_open_key: NULL argument");
+    Fr tau;
+    memcpy(tau.l, tau32, sizeof tau.l);
+    if (tau.is_zero()) return fail(ctx, DP_E_ARG, "dp_srs_open_key: tau is zero");
+    if (!tau.canon_is_reduced()) return fail(ctx, DP_E_ARG, "dp_srs_open_key: tau is not a canonical scalar (tau >= r)");
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    uint64_t *dev = tmp.get<uint64_t>(2 * 25);
+    if (!dev) return fail(ctx, DP_E_OOM, "dp_srs_open_key buffer");
+    DP_LAUNCH(g2_open_key_kernel, dim3(1), dim3(32), 0, ctx->stream, tau, dev);
+    ctx->launches++;
+    DP_CUDA(ctx, cudaMemcpyAsync(out400, dev, 2 * (size_t)DP_G2_AFFINE_BYTES, cudaMemcpyDeviceToHost, ctx->stream));
+    return call_end(ctx, true);
+}
+
+int dp_multi_pairing(dp_ctx *ctx, const void *g1_104, const void *g2_200, size_t k, void *out576) {
+    if (!ctx) return fail(ctx, DP_E_ARG, "dp_multi_pairing: ctx is NULL");
+    if (!out576 || (k && (!g1_104 || !g2_200))) return fail(ctx, DP_E_ARG, "dp_multi_pairing: NULL argument");
+    if (k > ((size_t)1 << 20)) return fail(ctx, DP_E_ARG, "dp_multi_pairing: %zu pairs exceed 2^20", k);
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    uint64_t *p = tmp.get<uint64_t>(k * 13), *q = tmp.get<uint64_t>(k * 25);
+    Fq12 *f = tmp.get<Fq12>(k), *out = tmp.get<Fq12>(1);
+    unsigned long long *bad = tmp.get<unsigned long long>(1), verdict = ~0ull;
+    if (!p || !q || !f || !out || !bad) return fail(ctx, DP_E_OOM, "dp_multi_pairing buffers for %zu pairs", k);
+    DP_CUDA(ctx, cudaMemcpyAsync(bad, &verdict, sizeof verdict, cudaMemcpyHostToDevice, ctx->stream));
+    if (k) {
+        DP_CUDA(ctx, cudaMemcpyAsync(p, g1_104, k * (size_t)DP_G1_AFFINE_BYTES, cudaMemcpyHostToDevice, ctx->stream));
+        DP_CUDA(ctx, cudaMemcpyAsync(q, g2_200, k * (size_t)DP_G2_AFFINE_BYTES, cudaMemcpyHostToDevice, ctx->stream));
+        DP_LAUNCH(pairing_miller_kernel, dim3(blocks_for(2 * (uint64_t)k, 64)), dim3(64), 0, ctx->stream, (const uint64_t *)p,
+                  (const uint64_t *)q, (uint32_t)k, f, bad);
+        ctx->launches++;
+    }
+    DP_LAUNCH(pairing_final_kernel, dim3(1), dim3(32), 0, ctx->stream, (const Fq12 *)f, (uint32_t)k, (const unsigned long long *)bad, out);
+    ctx->launches++;
+    DP_CUDA(ctx, cudaMemcpyAsync(&verdict, bad, sizeof verdict, cudaMemcpyDeviceToHost, ctx->stream));
+    DP_TRY(call_end(ctx, true));
+    if (verdict != ~0ull) {
+        static const char *const reason[] = {"", "a G1 coordinate is not below p", "the G1 point is not on the curve",
+                                             "a G2 coordinate is not below p", "the G2 point is not on the twist",
+                                             "the G2 point is not in the r-torsion subgroup"};
+        return fail(ctx, DP_E_ARG, "dp_multi_pairing: pair %llu rejected: %s", (unsigned long long)((verdict >> 8) - 1),
+                    reason[(verdict & 0xff) < 6 ? verdict & 0xff : 0]);
+    }
+    DP_CUDA(ctx, cudaMemcpy(out576, out, sizeof(Fq12), cudaMemcpyDeviceToHost));
+    return DP_OK;
 }
 
 int dp_debug_set_limits(dp_ctx *ctx, uint32_t max_contig_log_k, uint32_t max_strided_log_k, int msm_window_bits) {

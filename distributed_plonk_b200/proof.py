@@ -11,7 +11,8 @@ import numpy as np
 from .transcript import R_MOD
 
 FQ_MOD = 0x1A0111EA397FE69A4B1BA7B6434BACD764774B84F38512BF6730D2A0F6B0F6241EABFFFEB153FFFFB9FEFFFFFFFFAAAB
-_FQ_RINV = pow((1 << 384) % FQ_MOD, -1, FQ_MOD)
+_FQ_R = (1 << 384) % FQ_MOD
+_FQ_RINV = pow(_FQ_R, -1, FQ_MOD)
 _FR_R = (1 << 256) % R_MOD
 _FR_RINV = pow(_FR_R, -1, R_MOD)
 
@@ -36,6 +37,46 @@ def point_from_jacobian(raw) -> tuple | None:
     zi = pow(Z, -1, FQ_MOD)
     zi2 = zi * zi % FQ_MOD
     return X * zi2 % FQ_MOD, Y * zi2 * zi % FQ_MOD
+
+
+def _fq_raw(v: int) -> bytes:
+    return (int(v) % FQ_MOD * _FQ_R % FQ_MOD).to_bytes(48, "little")
+
+
+def _fq_from_raw(b: bytes) -> int:
+    return int.from_bytes(b, "little") * _FQ_RINV % FQ_MOD
+
+
+def point_to_raw(pt) -> bytes:
+    """affine canonical (x, y) or None -> raw ark GroupAffine<G1> (104 B: x, y Montgomery, infinity flag, padding);
+    the identity is (0, 1, true)"""
+    if pt is None:
+        return _fq_raw(0) + _fq_raw(1) + b"\x01" + bytes(7)
+    return _fq_raw(pt[0]) + _fq_raw(pt[1]) + bytes(8)
+
+
+def point_from_raw(raw) -> tuple | None:
+    """the inverse of point_to_raw"""
+    b = np.ascontiguousarray(raw, dtype=np.uint8).tobytes()
+    return None if b[96] else (_fq_from_raw(b[0:48]), _fq_from_raw(b[48:96]))
+
+
+def g2_to_raw(q) -> bytes:
+    """G2 point ((x.c0, x.c1), (y.c0, y.c1)) canonical ints, or None -> raw ark GroupAffine<G2> (200 B: x.c0, x.c1, y.c0,
+    y.c1 Montgomery, infinity flag, padding); the identity is (0, 1, true)"""
+    if q is None:
+        return _fq_raw(0) * 2 + _fq_raw(1) + _fq_raw(0) + b"\x01" + bytes(7)
+    (x0, x1), (y0, y1) = q
+    return b"".join(_fq_raw(v) for v in (x0, x1, y0, y1)) + bytes(8)
+
+
+def g2_from_raw(raw) -> tuple | None:
+    """the inverse of g2_to_raw"""
+    b = np.ascontiguousarray(raw, dtype=np.uint8).tobytes()
+    if b[192]:
+        return None
+    v = [_fq_from_raw(b[48 * i:48 * (i + 1)]) for i in range(4)]
+    return (v[0], v[1]), (v[2], v[3])
 
 
 def g1_compress(pt) -> bytes:

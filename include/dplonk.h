@@ -44,6 +44,8 @@ extern "C" {
 #define DP_G1_AFFINE_BYTES 104
 #define DP_G1_COMPRESSED_BYTES 48 /* ark-serialize 0.3.0 compressed GroupAffine */
 #define DP_G1_PROJECTIVE_BYTES 144
+#define DP_G2_AFFINE_BYTES 200     /* raw ark 0.3 GroupAffine<g2::Parameters>: x.c0, x.c1, y.c0, y.c1, infinity, padding */
+#define DP_FQ12_BYTES 576          /* 12 Montgomery Fq in the order of the tower Fq2 -> Fq6 -> Fq12 (DESIGN.md 3.8)      */
 
 typedef struct dp_ctx dp_ctx;
 
@@ -86,6 +88,25 @@ int dp_get_bases(dp_ctx *ctx, uint64_t start, size_t n, void *out104);
  * the context keeps until the next dp_init.  Returns when the points are written.  n = 0 writes nothing;
  * n > 2^32 is DP_E_ARG.  Whoever knows tau can forge proofs against this SRS.                             */
 int dp_srs_powers_of_tau(dp_ctx *ctx, const void *tau32, size_t n, void *out104);
+
+/* ---- verifier (DESIGN.md section 3.8): none of these needs dp_init; all read and write host memory ------------
+ * ark-serialize 0.3 compressed points (48 B each, the proof's encoding) -> raw G1Affine (104 B each), on the GPU.
+ * check_subgroup != 0 also runs the r-torsion check.  A rejected point returns DP_E_ARG, writes nothing to out104,
+ * and sets *bad_index to its index and *why to 1 (x >= p), 2 (both flag bits), 3 (no such point) or 4 (outside the
+ * subgroup); on success *bad_index = n and *why = 0 (either pointer may be NULL).                                  */
+int dp_g1_decompress(dp_ctx *ctx, const void *in48, size_t n, int check_subgroup, void *out104, size_t *bad_index, int *why);
+/* out144 = sum_i scalars32[i] * points104[i] over n caller-given raw G1Affine points (not validated; the identity
+ * flag is honoured).  Scalars: canonical BigInteger256 as in dp_msm.  out144: 144 B raw G1Projective, normalised
+ * (Z = 1) or the identity.  n = 0 writes the identity.                                                            */
+int dp_msm_points(dp_ctx *ctx, const void *points104, const void *scalars32, size_t n, void *out144);
+/* The G2 half of jf-plonk's KZG test setup: out400 = H, tau * H (two raw G2Affine, 200 B each), H the standard G2
+ * generator.  tau32: 32 B canonical, 0 < tau < r, else DP_E_ARG.                                                  */
+int dp_srs_open_key(dp_ctx *ctx, const void *tau32, void *out400);
+/* out576 = prod_i e(g1_104[i], g2_200[i]) as an Fq12 (DP_FQ12_BYTES), one final exponentiation for all k pairs.
+ * e(P, Q) = f^(3 (p^12 - 1) / r) for the optimal-ate Miller value f: the cube of the textbook reduced pairing
+ * (DESIGN.md section 3.8).  A pair with a point at infinity contributes 1; k = 0 gives 1.  A G1 point off the curve,
+ * a G2 point off the twist or outside the r-torsion, or a coordinate >= p is DP_E_ARG naming the first bad pair.   */
+int dp_multi_pairing(dp_ctx *ctx, const void *g1_104, const void *g2_200, size_t k, void *out576);
 
 /* ---- PlonkSlave.varMsm (src/worker.rs:159-185) -----------------------------------------------
  * out = sum_{k < min(end-start, n_scalars)} scalars[k] * bases[start + k]
