@@ -8,6 +8,7 @@ import numpy as np
 DP_OK, DP_E_ARG, DP_E_STATE, DP_E_OOM, DP_E_CUDA, DP_E_COMM = 0, -1, -2, -3, -4, -5
 FR_BYTES, G1_AFFINE_BYTES, G1_PROJECTIVE_BYTES = 32, 104, 144
 G1_COMPRESSED_BYTES, G2_AFFINE_BYTES, FQ12_BYTES = 48, 200, 576
+G2_COMPRESSED_BYTES = 96
 
 EXPORTS = [
     "dp_create", "dp_destroy", "dp_last_error", "dp_version", "dp_init", "dp_msm", "dp_commit", "dp_fft_init",
@@ -24,6 +25,7 @@ EXPORTS = [
     "dp_wire_permutation_scratch_bytes", "dp_wire_permutation_dev", "dp_perm_evals_dev", "dp_witness_gather_dev", "dp_commit_dev_batch",
     "dp_srs_powers_of_tau",
     "dp_g1_decompress", "dp_msm_points", "dp_srs_open_key", "dp_multi_pairing",
+    "dp_g1_compress", "dp_get_bases_compressed", "dp_g2_compress", "dp_g2_decompress", "dp_srs_check", "dp_last_srs_check",
 ]
 
 
@@ -125,6 +127,12 @@ def bind(cdll: C.CDLL) -> C.CDLL:
         "dp_msm_points": (i, [vp, vp, vp, sz, vp]),
         "dp_srs_open_key": (i, [vp, vp, vp]),
         "dp_multi_pairing": (i, [vp, vp, vp, sz, vp]),
+        "dp_g1_compress": (i, [vp, vp, sz, vp]),
+        "dp_get_bases_compressed": (i, [vp, u64, sz, vp]),
+        "dp_g2_compress": (i, [vp, vp, sz, vp]),
+        "dp_g2_decompress": (i, [vp, vp, sz, i, vp, C.POINTER(sz), C.POINTER(i)]),
+        "dp_srs_check": (i, [vp, vp, vp, C.POINTER(i)]),
+        "dp_last_srs_check": (i, [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), vp]),
         "dp_poly_eval": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_eval_dev": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_lincomb": (i, [vp, C.POINTER(vp), C.POINTER(sz), vp, sz, vp, sz]),
@@ -628,6 +636,63 @@ class Context:
         out = np.zeros(FQ12_BYTES, dtype=np.uint8)
         self._ck(self.lib.dp_multi_pairing(self.h, _addr(p) if k else None, _addr(q) if k else None, k, _addr(out)))
         return out
+
+    # ---- setup files (only get_bases_compressed and srs_check need init)
+    def g1_compress(self, points104) -> np.ndarray:
+        """[n, 104] raw G1Affine -> [n, 48] ark-serialize compressed points (the inverse of g1_decompress)"""
+        p = np.ascontiguousarray(points104, dtype=np.uint8).reshape(-1, G1_AFFINE_BYTES)
+        n = p.shape[0]
+        out = np.zeros((n, G1_COMPRESSED_BYTES), dtype=np.uint8)
+        self._ck(self.lib.dp_g1_compress(self.h, _addr(p) if n else None, n, _addr(out) if n else None))
+        return out
+
+    def get_bases_compressed(self, start: int, n: int, out: np.ndarray | None = None) -> np.ndarray:
+        """bases [start, start + n) as [n, 48] compressed points, into `out` when given"""
+        if out is None:
+            out = np.zeros((n, G1_COMPRESSED_BYTES), dtype=np.uint8)
+        assert out.dtype == np.uint8 and out.size == n * G1_COMPRESSED_BYTES
+        self._ck(self.lib.dp_get_bases_compressed(self.h, start, n, _addr(out) if n else None))
+        return out
+
+    def g2_compress(self, points200) -> np.ndarray:
+        """[n, 200] raw G2Affine -> [n, 96] ark-serialize compressed points"""
+        q = np.ascontiguousarray(points200, dtype=np.uint8).reshape(-1, G2_AFFINE_BYTES)
+        n = q.shape[0]
+        out = np.zeros((n, G2_COMPRESSED_BYTES), dtype=np.uint8)
+        self._ck(self.lib.dp_g2_compress(self.h, _addr(q) if n else None, n, _addr(out) if n else None))
+        return out
+
+    def g2_decompress(self, points96, check_subgroup: bool = True) -> np.ndarray:
+        """[n, 96] compressed points -> [n, 200] raw G2Affine.  A rejected point raises DpError with `index` and `why`
+        (1 a coordinate >= p, 2 both flags, 3 no such point, 4 outside the subgroup), as g1_decompress does"""
+        b = np.ascontiguousarray(points96, dtype=np.uint8).reshape(-1, G2_COMPRESSED_BYTES)
+        n = b.shape[0]
+        out = np.zeros((n, G2_AFFINE_BYTES), dtype=np.uint8)
+        idx, why = C.c_size_t(), C.c_int()
+        rc = self.lib.dp_g2_decompress(self.h, _addr(b) if n else None, n, int(check_subgroup), _addr(out) if n else None,
+                                       C.byref(idx), C.byref(why))
+        if rc != DP_OK:
+            err = DpError(rc, (self.lib.dp_last_error(self.h) or b"").decode())
+            err.index, err.why = idx.value, why.value
+            raise err
+        return out
+
+    def srs_check(self, g2_400, seed: bytes | None = None) -> bool:
+        """are the context's bases the powers of the tau of the open key (h, beta h: [2, 200] raw G2Affine)?  seed: 32 bytes
+        that make the random scalars reproducible; None lets the library draw them from the operating system"""
+        q = np.ascontiguousarray(g2_400, dtype=np.uint8).reshape(2, G2_AFFINE_BYTES)
+        if seed is not None and len(seed) != 32:
+            raise ValueError("the seed is 32 bytes")
+        ok = C.c_int()
+        self._ck(self.lib.dp_srs_check(self.h, _addr(q), bytes(seed) if seed is not None else None, C.byref(ok)))
+        return bool(ok.value)
+
+    def last_srs_check(self) -> dict:
+        """the last srs_check: {"scalars_ms", "msm_ms", "pairing_ms"} and its two MSM results "A", "B" (144 B each)"""
+        a, b, c = C.c_float(), C.c_float(), C.c_float()
+        ab = np.zeros((2, G1_PROJECTIVE_BYTES), dtype=np.uint8)
+        self._ck(self.lib.dp_last_srs_check(self.h, C.byref(a), C.byref(b), C.byref(c), _addr(ab)))
+        return {"scalars_ms": a.value, "msm_ms": b.value, "pairing_ms": c.value, "A": ab[0], "B": ab[1]}
 
     def init_ptr(self, bases_ptr: int, n_bases: int, domain_size: int, quot_domain_size: int):
         """PlonkSlave.init with the raw GroupAffine array at `bases_ptr` (host or device memory)"""

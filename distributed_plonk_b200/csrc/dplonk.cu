@@ -206,6 +206,9 @@ struct dp_ctx {
     uint32_t quot_inv_log = 0;
     // fixed-base table of dp_srs_powers_of_tau (srs.cuh, 48 MiB): built by its first call, dropped by the next dp_init
     G1Affine *srs_table = nullptr;
+    // the last dp_srs_check: ms of its scalar generation, two MSMs and pairing, and its two MSM results (dp_last_srs_check)
+    float srs_check_ms[3] = {0.f, 0.f, 0.f};
+    G1JacobianOut srs_check_ab[2] = {};
     // batched-affine tree levels in front of the XYZZ chunks (msm.cuh): 0 = none, else L.  env DP_MSM_AFFINE=L forces L levels;
     // otherwise dp_init chooses by msm_tune() - one MSM over the context's own window table per candidate, results compared
     // byte for byte, levels kept only if identical and faster (an SRS whose hot-path MSM has fewer than msm_affine_min_digits
@@ -2863,6 +2866,180 @@ int dp_multi_pairing(dp_ctx *ctx, const void *g1_104, const void *g2_200, size_t
                     reason[(verdict & 0xff) < 6 ? verdict & 0xff : 0]);
     }
     DP_CUDA(ctx, cudaMemcpy(out576, out, sizeof(Fq12), cudaMemcpyDeviceToHost));
+    return DP_OK;
+}
+
+// ---- setup files: the encoders, the G2 decoder and the consistency check of a loaded SRS (DESIGN.md section 3.9)
+// n points to 48 compressed bytes each, SRS_CHUNK points at a time: `src_dev` (resident 96-byte bases) or, when it is NULL,
+// the raw structs at in104 (host or device memory), staged chunk by chunk
+static int g1_compress_chunks(dp_ctx *ctx, const G1Affine *src_dev, const void *in104, size_t n, void *out48, const char *who) {
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    const uint64_t chunk = n < SRS_CHUNK ? n : SRS_CHUNK;
+    uint32_t *packed = tmp.get<uint32_t>(chunk * 12);
+    uint64_t *raw = src_dev ? nullptr : tmp.get<uint64_t>(chunk * 13);
+    if (!packed || (!src_dev && !raw)) return fail(ctx, DP_E_OOM, "%s buffers", who);
+    for (uint64_t first = 0; first < n; first += chunk) {
+        const uint64_t m = first + chunk < n ? chunk : n - first;
+        if (src_dev) {
+            DP_LAUNCH(g1_compress_kernel, dim3(blocks_for(m, 256)), dim3(256), 0, ctx->stream, src_dev + first, packed, m);
+        } else {
+            DP_CUDA(ctx, cudaMemcpyAsync(raw, (const uint8_t *)in104 + first * DP_G1_AFFINE_BYTES, m * DP_G1_AFFINE_BYTES, cudaMemcpyDefault,
+                                         ctx->stream));
+            DP_LAUNCH(g1_compress_ark_kernel, dim3(blocks_for(m, 256)), dim3(256), 0, ctx->stream, (const uint64_t *)raw, packed, m);
+        }
+        ctx->launches++;
+        DP_CUDA(ctx, cudaMemcpyAsync((uint8_t *)out48 + first * DP_G1_COMPRESSED_BYTES, packed, m * DP_G1_COMPRESSED_BYTES, cudaMemcpyDefault,
+                                     ctx->stream));
+    }
+    return call_end(ctx, true);
+}
+
+int dp_g1_compress(dp_ctx *ctx, const void *in104, size_t n, void *out48) {
+    if (!ctx) return fail(ctx, DP_E_ARG, "dp_g1_compress: ctx is NULL");
+    if (n && (!in104 || !out48)) return fail(ctx, DP_E_ARG, "dp_g1_compress: NULL argument");
+    if (n == 0) return DP_OK;
+    return g1_compress_chunks(ctx, nullptr, in104, n, out48, "dp_g1_compress");
+}
+
+int dp_get_bases_compressed(dp_ctx *ctx, uint64_t start, size_t n, void *out48) {
+    if (!ctx || (n && !out48)) return fail(ctx, DP_E_ARG, "dp_get_bases_compressed: NULL argument");
+    if (!ctx->inited) return fail(ctx, DP_E_STATE, "dp_get_bases_compressed before dp_init");
+    if (start > ctx->n_bases || n > ctx->n_bases - start)
+        return fail(ctx, DP_E_ARG, "dp_get_bases_compressed: range outside %llu bases", (unsigned long long)ctx->n_bases);
+    if (n == 0) return DP_OK;
+    return g1_compress_chunks(ctx, ctx->bases + start, nullptr, n, out48, "dp_get_bases_compressed");
+}
+
+int dp_g2_compress(dp_ctx *ctx, const void *in200, size_t n, void *out96) {
+    if (!ctx) return fail(ctx, DP_E_ARG, "dp_g2_compress: ctx is NULL");
+    if (n && (!in200 || !out96)) return fail(ctx, DP_E_ARG, "dp_g2_compress: NULL argument");
+    if (n > ((size_t)1 << 20)) return fail(ctx, DP_E_ARG, "dp_g2_compress: %zu points exceed 2^20", n);
+    if (n == 0) return DP_OK;
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    uint64_t *raw = tmp.get<uint64_t>(n * 25);
+    uint32_t *packed = tmp.get<uint32_t>(n * 24);
+    if (!raw || !packed) return fail(ctx, DP_E_OOM, "dp_g2_compress buffers");
+    DP_CUDA(ctx, cudaMemcpyAsync(raw, in200, n * (size_t)DP_G2_AFFINE_BYTES, cudaMemcpyDefault, ctx->stream));
+    DP_LAUNCH(g2_compress_kernel, dim3(blocks_for(n, 32)), dim3(32), 0, ctx->stream, (const uint64_t *)raw, packed, (uint64_t)n);
+    ctx->launches++;
+    DP_CUDA(ctx, cudaMemcpyAsync(out96, packed, n * (size_t)DP_G2_COMPRESSED_BYTES, cudaMemcpyDefault, ctx->stream));
+    return call_end(ctx, true);
+}
+
+int dp_g2_decompress(dp_ctx *ctx, const void *in96, size_t n, int check_subgroup, void *out200, size_t *bad_index, int *why) {
+    if (!ctx) return fail(ctx, DP_E_ARG, "dp_g2_decompress: ctx is NULL");
+    if (n && (!in96 || !out200)) return fail(ctx, DP_E_ARG, "dp_g2_decompress: NULL argument");
+    if (n > ((size_t)1 << 20)) return fail(ctx, DP_E_ARG, "dp_g2_decompress: %zu points exceed 2^20", n);
+    if (bad_index) *bad_index = n;
+    if (why) *why = 0;
+    if (n == 0) return DP_OK;
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    uint32_t *packed = tmp.get<uint32_t>(n * 24);
+    uint64_t *raw = tmp.get<uint64_t>(n * 25);
+    unsigned long long *err = tmp.get<unsigned long long>(1), verdict = ~0ull;
+    if (!packed || !raw || !err) return fail(ctx, DP_E_OOM, "dp_g2_decompress buffers");
+    DP_CUDA(ctx, cudaMemcpyAsync(packed, in96, n * (size_t)DP_G2_COMPRESSED_BYTES, cudaMemcpyDefault, ctx->stream));
+    DP_CUDA(ctx, cudaMemcpyAsync(err, &verdict, sizeof verdict, cudaMemcpyHostToDevice, ctx->stream));
+    DP_LAUNCH(g2_decompress_kernel, dim3(blocks_for(n, 32)), dim3(32), 0, ctx->stream, (const uint32_t *)packed, raw, (uint64_t)n,
+              check_subgroup ? 1u : 0u, err);
+    ctx->launches++;
+    DP_CUDA(ctx, cudaMemcpyAsync(&verdict, err, sizeof verdict, cudaMemcpyDeviceToHost, ctx->stream));
+    DP_TRY(call_end(ctx, true));
+    if (verdict != ~0ull) {
+        const size_t idx = (size_t)((verdict >> 8) - 1);
+        if (bad_index) *bad_index = idx;
+        if (why) *why = (int)(verdict & 7);
+        static const char *const reason[] = {"", "a coordinate is not a canonical field element", "both flag bits set",
+                                             "x^3 + 4 (u + 1) is not a square: no such point", "the point is not in the r-torsion subgroup"};
+        return fail(ctx, DP_E_ARG, "dp_g2_decompress: point %zu rejected: %s", idx, reason[verdict & 7]);
+    }
+    DP_CUDA(ctx, cudaMemcpy(out200, raw, n * (size_t)DP_G2_AFFINE_BYTES, cudaMemcpyDefault));
+    return DP_OK;
+}
+
+int dp_srs_check(dp_ctx *ctx, const void *g2_400, const void *seed32, int *ok) {
+    if (!ctx) return fail(ctx, DP_E_ARG, "dp_srs_check: ctx is NULL");
+    if (!g2_400 || !ok) return fail(ctx, DP_E_ARG, "dp_srs_check: NULL argument");
+    if (!ctx->inited) return fail(ctx, DP_E_STATE, "dp_srs_check before dp_init");
+    const uint64_t n = ctx->n_bases;
+    if (n == 0) return fail(ctx, DP_E_STATE, "dp_srs_check: the context holds no bases");
+    *ok = 0;
+    ChaChaKey key;
+    if (seed32) {
+        memcpy(key.w, seed32, sizeof key.w);
+    } else {
+        size_t got = 0;
+        while (got < sizeof key.w) {
+            const ssize_t r = getrandom(reinterpret_cast<uint8_t *>(key.w) + got, sizeof key.w - got, 0);
+            if (r < 0) return fail(ctx, DP_E_STATE, "dp_srs_check: getrandom failed; pass a seed");
+            got += (size_t)r;
+        }
+    }
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    using clock = std::chrono::steady_clock;
+    auto ms_since = [](clock::time_point t0) { return std::chrono::duration<float, std::milli>(clock::now() - t0).count(); };
+    for (float &v : ctx->srs_check_ms) v = 0.f;
+    ctx->srs_check_ab[0] = ctx->srs_check_ab[1] = G1JacobianOut::from_affine(G1Affine::inf());
+    G1Affine first;
+    DP_CUDA(ctx, cudaMemcpy(&first, ctx->bases, sizeof first, cudaMemcpyDeviceToHost));
+    const G1Affine gen = g1_generator();
+    if (!(first.x == gen.x) || !(first.y == gen.y)) return DP_OK;  // P_0 is not the generator
+    if (n == 1) {
+        *ok = 1;
+        return DP_OK;
+    }
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    uint4 *sa = tmp.get<uint4>(2 * n), *sb = tmp.get<uint4>(2 * n);
+    G1JacobianOut *od = tmp.get<G1JacobianOut>(2);
+    if (!sa || !sb || !od) return fail(ctx, DP_E_OOM, "dp_srs_check: scalars for %llu bases", (unsigned long long)n);
+    clock::time_point t0 = clock::now();
+    DP_LAUNCH(srs_check_scalars_kernel, dim3(blocks_for((n + 2) / 4, 128)), dim3(128), 0, ctx->stream, key, n, sa, sb);
+    ctx->launches++;
+    DP_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->srs_check_ms[0] = ms_since(t0);
+    // both over the whole SRS from base 0, the range the window-multiple table of dp_init covers
+    t0 = clock::now();
+    DP_TRY(msm_device(ctx, 0, sa, n, od, nullptr));
+    DP_TRY(msm_device(ctx, 0, sb, n, od + 1, nullptr));
+    DP_CUDA(ctx, cudaMemcpyAsync(ctx->srs_check_ab, od, 2 * sizeof(G1JacobianOut), cudaMemcpyDeviceToHost, ctx->stream));
+    DP_TRY(call_end(ctx, true));
+    ctx->srs_check_ms[1] = ms_since(t0);
+    // e(A, beta h) * e(-B, h) == 1  <=>  sum rho_i (tau P_i - P_(i+1)) == 0
+    t0 = clock::now();
+    uint8_t g1[2 * DP_G1_AFFINE_BYTES] = {};  // raw structs: the limbs of a Montgomery Fq are its 48 little-endian bytes
+    for (int k = 0; k < 2; k++) {
+        const G1JacobianOut &j = ctx->srs_check_ab[k];
+        const bool inf = j.z.is_zero();
+        const Fq x = inf ? Fq::zero() : j.x, y = inf ? Fq::one() : k == 0 ? j.y : j.y.neg();
+        memcpy(g1 + DP_G1_AFFINE_BYTES * k, x.l, 48);
+        memcpy(g1 + DP_G1_AFFINE_BYTES * k + 48, y.l, 48);
+        g1[DP_G1_AFFINE_BYTES * k + 96] = inf ? 1 : 0;
+    }
+    uint8_t pair[2 * DP_G2_AFFINE_BYTES];
+    memcpy(pair, (const uint8_t *)g2_400 + DP_G2_AFFINE_BYTES, DP_G2_AFFINE_BYTES);  // beta h pairs with A
+    memcpy(pair + DP_G2_AFFINE_BYTES, g2_400, DP_G2_AFFINE_BYTES);                   // h with -B
+    uint8_t e[DP_FQ12_BYTES], one[DP_FQ12_BYTES] = {};  // 1 in Fq12: the first of the 12 coefficients is 1
+    const Fq fq_one = Fq::one();
+    memcpy(one, fq_one.l, 48);
+    DP_TRY(dp_multi_pairing(ctx, g1, pair, 2, e));
+    ctx->srs_check_ms[2] = ms_since(t0);
+    *ok = memcmp(e, one, sizeof e) == 0 ? 1 : 0;
+    return DP_OK;
+}
+
+int dp_last_srs_check(const dp_ctx *ctx, float *scalars_ms, float *msm_ms, float *pairing_ms, void *ab288) {
+    if (!ctx) return DP_E_ARG;
+    if (scalars_ms) *scalars_ms = ctx->srs_check_ms[0];
+    if (msm_ms) *msm_ms = ctx->srs_check_ms[1];
+    if (pairing_ms) *pairing_ms = ctx->srs_check_ms[2];
+    if (ab288) memcpy(ab288, ctx->srs_check_ab, sizeof ctx->srs_check_ab);
     return DP_OK;
 }
 

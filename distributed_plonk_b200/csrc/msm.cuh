@@ -209,6 +209,92 @@ __global__ void __launch_bounds__(128) g1_decompress_kernel(const uint32_t *in, 
     out[i] = p;
 }
 
+// The inverse of g1_decompress_kernel: device affine -> the 48 compressed bytes (12 u32).  Two Montgomery reductions
+// per point (x and y leave Montgomery form; -y is then p - y on the canonical integer), so 96 or 104 B read and 48 B
+// written per point against ~300 multiply-adds: the kernels below are meant to run at the speed of their memory traffic.
+DP_D void g1_compress_store(const G1Affine &p, uint32_t *out) {
+    Fq x = Fq::zero();
+    uint32_t flags = 1u << 30;
+    if (!p.is_inf()) {
+        x = p.x.from_mont();
+        const Fq y = p.y.from_mont();
+        flags = Fq::canon_gt(y, y.neg()) ? 1u << 31 : 0u;
+    }
+#pragma unroll
+    for (int k = 0; k < 12; k++) out[k] = x.l[k] | (k == 11 ? flags : 0u);
+}
+// from the context's resident bases (96 B each)
+__global__ void __launch_bounds__(256) g1_compress_kernel(const G1Affine *in, uint32_t *out, uint64_t n) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) g1_compress_store(in[i], out + i * 12);
+}
+// from raw ark GroupAffine structs (104 B each, the layout g1_import_ark_kernel reads; not validated)
+__global__ void __launch_bounds__(256) g1_compress_ark_kernel(const uint64_t *ark, uint32_t *out, uint64_t n) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t *src = ark + i * 13;
+    G1Affine p = G1Affine::inf();
+    if ((src[12] & 0xff) == 0) {
+#pragma unroll
+        for (int k = 0; k < 6; k++) {
+            p.x.l[2 * k] = (uint32_t)src[k];
+            p.x.l[2 * k + 1] = (uint32_t)(src[k] >> 32);
+            p.y.l[2 * k] = (uint32_t)src[6 + k];
+            p.y.l[2 * k + 1] = (uint32_t)(src[6 + k] >> 32);
+        }
+    }
+    g1_compress_store(p, out + i * 12);
+}
+
+// The random scalars of dp_srs_check: rho_i = 128 bits, words 4 (i mod 4) .. 4 (i mod 4) + 3 (little-endian) of the
+// ChaCha20 block (RFC 8439 section 2.3) with the 256-bit key `key`, block counter i div 4 and an all-zero nonce.
+DP_D void chacha20_block(const uint32_t *key, uint32_t counter, uint32_t *out) {
+    uint32_t s[16] = {0x61707865u, 0x3320646eu, 0x79622d32u, 0x6b206574u, key[0], key[1], key[2], key[3],
+                      key[4],      key[5],      key[6],      key[7],      counter, 0u,     0u,     0u};
+    uint32_t x[16];
+#pragma unroll
+    for (int k = 0; k < 16; k++) x[k] = s[k];
+    auto rotl = [](uint32_t v, int c) { return (v << c) | (v >> (32 - c)); };
+    auto quarter = [&](int a, int b, int c, int d) {
+        x[a] += x[b]; x[d] = rotl(x[d] ^ x[a], 16);
+        x[c] += x[d]; x[b] = rotl(x[b] ^ x[c], 12);
+        x[a] += x[b]; x[d] = rotl(x[d] ^ x[a], 8);
+        x[c] += x[d]; x[b] = rotl(x[b] ^ x[c], 7);
+    };
+    for (int round = 0; round < 10; round++) {
+        quarter(0, 4, 8, 12); quarter(1, 5, 9, 13); quarter(2, 6, 10, 14); quarter(3, 7, 11, 15);
+        quarter(0, 5, 10, 15); quarter(1, 6, 11, 12); quarter(2, 7, 8, 13); quarter(3, 4, 9, 14);
+    }
+#pragma unroll
+    for (int k = 0; k < 16; k++) out[k] = x[k] + s[k];
+}
+struct ChaChaKey {
+    uint32_t w[8];
+};
+// One thread per block = four scalars.  a[i] = rho_i and b[i + 1] = rho_i for i < n - 1, a[n - 1] = b[0] = 0: canonical
+// 256-bit MSM scalars (two uint4 each), so that sum a[i] P_i and sum b[i] P_i pair rho_i with P_i and with P_(i+1).
+__global__ void __launch_bounds__(128) srs_check_scalars_kernel(ChaChaKey key, uint64_t n, uint4 *a, uint4 *b) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint4 zero = make_uint4(0, 0, 0, 0);
+    if (t == 0) {
+        a[2 * (n - 1)] = a[2 * (n - 1) + 1] = zero;
+        b[0] = b[1] = zero;
+    }
+    if (4 * t >= n - 1) return;
+    uint32_t ks[16];
+    chacha20_block(key.w, (uint32_t)t, ks);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+        const uint64_t i = 4 * t + j;
+        if (i >= n - 1) break;
+        const uint4 rho = make_uint4(ks[4 * j], ks[4 * j + 1], ks[4 * j + 2], ks[4 * j + 3]);
+        a[2 * i] = rho;
+        a[2 * i + 1] = zero;
+        b[2 * (i + 1)] = rho;
+        b[2 * (i + 1) + 1] = zero;
+    }
+}
+
 // Synthetic SRS for benchmarks / tests: out[i] = k_i * G with k_i = SplitMix64(seed, i) (64-bit,
 // distinct points), written in the raw ark GroupAffine layout (104 B) that dp_init ingests.
 DP_HD G1Affine g1_generator() {

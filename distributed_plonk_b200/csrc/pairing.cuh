@@ -404,4 +404,113 @@ __global__ void __launch_bounds__(32) g2_open_key_kernel(Fr tau, uint64_t *out) 
     store_g2_ark(out + 25, g2_mul(h, tau.l).to_affine());
 }
 
+// ------------------------------------------------------------------------------------------------ compressed G2 points
+// ark-serialize 0.3 of GroupAffine<g2::Parameters>, 96 B = 24 u32: canonical x.c0 then x.c1, 48 little-endian bytes each;
+// bit 7 of the last byte = (y > -y), bit 6 = infinity.  Fq2 is ordered by c1 first, then c0 (canonical integers).
+DP_D bool fq2_is_larger_than_neg(const Fq2 &y) {  // Montgomery form; false for y = 0
+    const Fq c1 = y.c1.from_mont();
+    if (!c1.is_zero()) return Fq::canon_gt(c1, c1.neg());  // p is odd: c1 != -c1
+    const Fq c0 = y.c0.from_mont();
+    return Fq::canon_gt(c0, c0.neg());
+}
+
+// One thread per point; a file holds two of them.
+__global__ void __launch_bounds__(32) g2_compress_kernel(const uint64_t *in, uint32_t *out, uint64_t n) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const G2Affine q = load_g2_ark(in + i * 25);
+    Fq x0 = Fq::zero(), x1 = Fq::zero();
+    uint32_t flags = 1u << 30;
+    if (!q.inf) {
+        x0 = q.x.c0.from_mont();
+        x1 = q.x.c1.from_mont();
+        flags = fq2_is_larger_than_neg(q.y) ? 1u << 31 : 0u;
+    }
+    uint32_t *o = out + i * 24;
+#pragma unroll
+    for (int k = 0; k < 12; k++) {
+        o[k] = x0.l[k];
+        o[12 + k] = x1.l[k] | (k == 11 ? flags : 0u);
+    }
+}
+
+// a^((p + 1) / 4): a square root of a when a is a square, of -a otherwise (p = 3 mod 4; g1_decompress_kernel's exponent)
+DP_D Fq fq_sqrt_candidate(const Fq &a) {
+    uint32_t e[12];  // the low limb ...aaab + 1 does not carry
+#pragma unroll
+    for (int k = 0; k < 12; k++) e[k] = FqParams::mod(k);
+    e[0] += 1;
+#pragma unroll
+    for (int k = 0; k < 12; k++) e[k] = (e[k] >> 2) | (k < 11 ? e[k + 1] << 30 : 0);
+    return a.pow_limbs(e, 12);
+}
+// A square root of a in Fq2 = Fq[u]/(u^2 + 1), if there is one.  a = (x0 + x1 u)^2 means x0^2 - x1^2 = a0 and 2 x0 x1 = a1,
+// so x0^2 = (a0 +- alpha) / 2 with alpha^2 = a0^2 + a1^2, the norm.  With d = (a0 + alpha) / 2 and c = d^((p + 1) / 4):
+// c^2 = d gives x0 = c, x1 = a1 / (2c); c^2 = -d (d is not a square, so the other sign is: their product is -a1^2 / 4)
+// gives x1 = c, x0 = a1 / (2c).  Two exponentiations and one inversion; the caller squares the result to find out
+// whether a was a square at all.  a1 = 0: c = a0^((p + 1) / 4) is the root itself, or u times it.
+DP_D Fq2 fq2_sqrt_candidate(const Fq2 &a) {
+    if (a.c1.is_zero()) {
+        const Fq c = fq_sqrt_candidate(a.c0);
+        return c.sqr() == a.c0 ? Fq2{c, Fq::zero()} : Fq2{Fq::zero(), c};
+    }
+    const Fq alpha = fq_sqrt_candidate(a.c0.sqr() + a.c1.sqr());
+    Fq half = Fq::zero();  // (p + 1) / 2 = 1 / 2
+#pragma unroll
+    for (int k = 0; k < 12; k++) half.l[k] = FqParams::mod(k);
+    half.l[0] += 1;
+#pragma unroll
+    for (int k = 0; k < 12; k++) half.l[k] = (half.l[k] >> 1) | (k < 11 ? half.l[k + 1] << 31 : 0);
+    const Fq d = (a.c0 + alpha) * half.to_mont();
+    const Fq c = fq_sqrt_candidate(d);
+    if (c.is_zero()) return Fq2::zero();  // only when the norm is no square (then a is none either): d = 0 needs alpha = -a0
+    const Fq other = a.c1 * c.dbl().inverse_vartime();
+    return c.sqr() == d ? Fq2{c, other} : Fq2{other, c};
+}
+
+// One lane per point.  Reason codes as g1_decompress_kernel's: 1 a coordinate >= p, 2 both flags, 3 x^3 + 4 (u + 1) is not
+// a square, 4 outside the r-torsion; *err = min((index + 1) << 8 | why).  Writes the raw 200-byte struct.
+__global__ void __launch_bounds__(32) g2_decompress_kernel(const uint32_t *in, uint64_t *out, uint64_t n, uint32_t check_subgroup,
+                                                           unsigned long long *err) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Fq x0, x1;
+#pragma unroll
+    for (int k = 0; k < 12; k++) {
+        x0.l[k] = in[i * 24 + k];
+        x1.l[k] = in[i * 24 + 12 + k];
+    }
+    const bool positive = (x1.l[11] >> 31) & 1, infinity = (x1.l[11] >> 30) & 1;
+    x1.l[11] &= 0x3fffffffu;
+    uint32_t why = 0;
+    G2Affine q{Fq2::zero(), Fq2::one(), true};
+    if (positive && infinity) {
+        why = 2;
+    } else if (!infinity) {
+        if (!x0.canon_is_reduced() || !x1.canon_is_reduced()) {
+            why = 1;
+        } else {
+            const Fq2 x{x0.to_mont(), x1.to_mont()};
+            const Fq2 rhs = fq2_sqr(x) * x + g2_b();
+            const Fq2 y = fq2_sqrt_candidate(rhs);
+            if (!(fq2_sqr(y) == rhs)) {
+                why = 3;
+            } else {
+                q = G2Affine{x, fq2_is_larger_than_neg(y) == positive ? y : y.neg(), false};
+                if (check_subgroup) {
+                    uint32_t r[8];
+#pragma unroll
+                    for (int k = 0; k < 8; k++) r[k] = FrParams::mod(k);
+                    if (!g2_mul(q, r).is_inf()) why = 4;
+                }
+            }
+        }
+    }
+    if (why) {
+        atomicMin(err, ((unsigned long long)(i + 1) << 8) | why);
+        q = G2Affine{Fq2::zero(), Fq2::one(), true};
+    }
+    store_g2_ark(out + i * 25, q);
+}
+
 }  // namespace dp

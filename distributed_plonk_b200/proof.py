@@ -91,6 +91,61 @@ def g1_compress(pt) -> bytes:
     return bytes(b)
 
 
+def g2_compress(q) -> bytes:
+    """ark-serialize 0.3 compressed G2 point (96 B): x.c0 then x.c1, 48 little-endian bytes each; bit 7 of the last byte
+    set when y > -y (Fq2 ordered by c1 first, then c0), bit 6 for the identity - the format dp_g2_decompress reads"""
+    if q is None:
+        return bytes(95) + bytes([1 << 6])
+    (x0, x1), (y0, y1) = q
+    b = bytearray(int(x0).to_bytes(48, "little") + int(x1).to_bytes(48, "little"))
+    if (y1, y0) > ((-y1) % FQ_MOD, (-y0) % FQ_MOD):
+        b[95] |= 1 << 7
+    return bytes(b)
+
+
+_DECOMPRESS_WHY = {1: "a coordinate is not below p", 2: "both flag bits set", 3: "not a point of the curve", 4: "not in the r-torsion subgroup"}
+N_K, N_SELECTORS, N_SIGMAS = 5, 13, 5
+
+
+def decompress_points(ctx, encodings, what: str) -> list:
+    """compressed G1 points (48 B each) -> affine (x, y) or None, decoded and checked to lie in the r-torsion subgroup on the
+    GPU (dp_g1_decompress); ValueError naming the first rejected point"""
+    from ._binding import DP_E_ARG, DpError
+    try:
+        raw = ctx.g1_decompress(np.frombuffer(b"".join(encodings), dtype=np.uint8).reshape(len(encodings), 48), check_subgroup=True)
+    except DpError as e:
+        if e.code != DP_E_ARG:
+            raise
+        raise ValueError(f"point {e.index} of {what}: {_DECOMPRESS_WHY.get(e.why, e.msg)}") from e
+    return [point_from_raw(r) for r in raw]
+
+
+class _Reader:
+    """the bytes of an ark-serialize record, taken front to back; ValueError when they run out or are left over"""
+
+    def __init__(self, b, what: str):
+        self.b, self.off, self.what = bytes(b), 0, what
+
+    def take(self, k: int) -> bytes:
+        if self.off + k > len(self.b):
+            raise ValueError(f"truncated {self.what}: {len(self.b)} bytes")
+        self.off += k
+        return self.b[self.off - k:self.off]
+
+    def u64(self) -> int:
+        return struct.unpack("<Q", self.take(8))[0]
+
+    def vec(self, expected: int, size: int, name: str) -> list:
+        n = self.u64()
+        if n != expected:
+            raise ValueError(f"{self.what}: {name} has {n} entries, expected {expected}")
+        return [self.take(size) for _ in range(n)]
+
+    def end(self):
+        if self.off != len(self.b):
+            raise ValueError(f"{len(self.b) - self.off} trailing bytes after the {self.what}")
+
+
 @dataclass
 class VerifyingKey:
     """what a verifier needs of a circuit: the gate-domain size n, the number of public inputs, the coset representatives
@@ -100,6 +155,34 @@ class VerifyingKey:
     k: list
     selector_comms: list
     sigma_comms: list
+
+    def to_bytes(self) -> bytes:
+        """The fields in the order above under ark-serialize 0.3 conventions: n and num_inputs as u64 LE, each vector a
+        u64 LE length then its items, k as 32 canonical bytes each, points compressed (48 B).  1064 bytes.  This is this
+        library's own record: jf-plonk's VerifyingKey lists different fields from version to version."""
+        vec = lambda items, enc: struct.pack("<Q", len(items)) + b"".join(enc(x) for x in items)
+        return (struct.pack("<QQ", self.n, self.num_inputs) + vec(self.k, lambda v: int(v).to_bytes(32, "little"))
+                + vec(self.selector_comms, g1_compress) + vec(self.sigma_comms, g1_compress))
+
+    @classmethod
+    def from_bytes(cls, ctx, b) -> "VerifyingKey":
+        """The inverse of to_bytes.  The 18 points are decompressed and checked to lie in the r-torsion subgroup on the GPU
+        (dp_g1_decompress; ctx needs no init).  ValueError on a truncated input, trailing bytes, vector lengths other than
+        5 / 13 / 5, a k >= r, n not a power of two (or above 2^32, the field's largest domain), num_inputs > n, or a rejected point."""
+        r = _Reader(b, "verifying key")
+        n, num_inputs = r.u64(), r.u64()
+        k = [int.from_bytes(v, "little") for v in r.vec(N_K, 32, "k")]
+        comp = r.vec(N_SELECTORS, 48, "selector_comms") + r.vec(N_SIGMAS, 48, "sigma_comms")
+        r.end()
+        if n == 0 or n & (n - 1) or n > 1 << 32:
+            raise ValueError(f"verifying key: n = {n} is not a power of two up to 2^32")
+        if num_inputs > n:
+            raise ValueError(f"verifying key: {num_inputs} public inputs exceed n = {n}")
+        for i, v in enumerate(k):
+            if v >= R_MOD:
+                raise ValueError(f"verifying key: k[{i}] is not below r")
+        p = decompress_points(ctx, comp, "the verifying key")
+        return cls(n, num_inputs, k, p[:N_SELECTORS], p[N_SELECTORS:])
 
 
 @dataclass

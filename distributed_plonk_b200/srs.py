@@ -2,11 +2,18 @@
 the open key (g, h, beta h) a verifier needs."""
 from __future__ import annotations
 
+import os
 import secrets
+import struct
 from dataclasses import dataclass
 
-from .proof import g2_from_raw
+import numpy as np
+
+from ._binding import DP_E_ARG, DpError
+from .proof import _DECOMPRESS_WHY, _Reader, decompress_points, g1_compress, g2_compress, g2_from_raw, g2_to_raw
 from .transcript import R_MOD
+
+SAVE_CHUNK = 1 << 20            # points per dp_get_bases_compressed call of save_srs (48 MiB of host memory)
 
 # the standard G1 generator (ark-bls12-381 G1Affine::prime_subgroup_generator), affine canonical
 G1_GEN = (0x17F1D3A73197D7942695638C4FA9AC0FC3688C4F9774B905A14E3A3F171BAC586C55E83FF97A1AEFFB3AF00ADB22C6BB,
@@ -20,6 +27,10 @@ class OpenKey:
     g: tuple
     h: tuple
     beta_h: tuple
+
+    def to_bytes(self) -> bytes:
+        """g (48 B), h (96 B), beta_h (96 B) as ark-serialize 0.3 compressed points: 240 bytes"""
+        return g1_compress(self.g) + g2_compress(self.h) + g2_compress(self.beta_h)
 
 
 def universal_setup(ctx, torch, max_degree: int, domain_size: int, quot_domain_size: int, tau: int | None = None,
@@ -50,3 +61,99 @@ def open_key(ctx, tau: int) -> OpenKey:
     (dp_srs_open_key); needs no init.  Publish it with the SRS and forget tau."""
     h, beta_h = ctx.srs_open_key(tau)
     return OpenKey(G1_GEN, g2_from_raw(h), g2_from_raw(beta_h))
+
+
+def _g2_pair_from_bytes(ctx, b: bytes, what: str) -> tuple:
+    """h, beta_h from 2 x 96 compressed bytes, decoded and subgroup-checked on the GPU (dp_g2_decompress)"""
+    try:
+        raw = ctx.g2_decompress(np.frombuffer(b, dtype=np.uint8).reshape(2, 96), check_subgroup=True)
+    except DpError as e:
+        if e.code != DP_E_ARG:
+            raise
+        raise ValueError(f"{('h', 'beta_h')[e.index]} of {what}: {_DECOMPRESS_WHY.get(e.why, e.msg)}") from e
+    return g2_from_raw(raw[0]), g2_from_raw(raw[1])
+
+
+def open_key_from_bytes(ctx, b) -> OpenKey:
+    """The inverse of OpenKey.to_bytes; the three points are decoded and subgroup-checked on the GPU (ctx needs no init).
+    ValueError on a length other than 240 or a rejected point."""
+    r = _Reader(b, "open key")
+    g, g2 = r.take(48), r.take(192)
+    r.end()
+    h, beta_h = _g2_pair_from_bytes(ctx, g2, "the open key")
+    return OpenKey(decompress_points(ctx, [g], "the open key")[0], h, beta_h)
+
+
+def _n_bases(ctx) -> int:
+    """how many bases the initialised context holds: the largest start an empty range may have (an empty
+    dp_get_bases_compressed returns before it touches the device)"""
+    lo, hi = 0, 1 << 32
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        try:
+            ctx.get_bases_compressed(mid, 0)
+            lo = mid
+        except DpError as e:
+            if e.code != DP_E_ARG:
+                raise
+            hi = mid - 1
+    return lo
+
+
+def save_srs(ctx, path, open_key: OpenKey) -> int:
+    """Write the context's SRS and the G2 half of `open_key` as jf-plonk's UniversalSrs under ark-serialize 0.3
+    CanonicalSerialize: the number of G1 points (u64 LE), the points compressed (48 B each), then h and beta_h (96 B each).
+    The points are encoded on the GPU from the resident bases (dp_get_bases_compressed), SAVE_CHUNK at a time.  Returns
+    the number of points.  The file holds no secret."""
+    n = _n_bases(ctx)
+    if n == 0:
+        raise ValueError("the context holds no bases to save")
+    g2 = ctx.g2_compress(np.frombuffer(g2_to_raw(open_key.h) + g2_to_raw(open_key.beta_h), dtype=np.uint8).reshape(2, 200))
+    buf = np.empty((min(n, SAVE_CHUNK), 48), dtype=np.uint8)
+    with open(path, "wb") as f:
+        f.write(struct.pack("<Q", n))
+        for first in range(0, n, SAVE_CHUNK):
+            m = min(SAVE_CHUNK, n - first)
+            f.write(ctx.get_bases_compressed(first, m, buf[:m]).data)
+        f.write(g2.tobytes())
+    return n
+
+
+def load_srs(ctx, path, domain_size: int, quot_domain_size: int, check_subgroup: bool = True, check: bool = True) -> OpenKey:
+    """dp_init the context from a file save_srs wrote (or jf-plonk's UniversalSrs::serialize) and return its open key.
+
+    Every point is decompressed on the GPU; with check_subgroup (the default) every G1 point is also tested to lie in the
+    r-torsion subgroup, as the two G2 points always are.  With check (the default) dp_srs_check then tests that the G1
+    points are consecutive powers of the tau of (h, beta_h), starting at the generator - whoever wrote the file cannot
+    predict the test's random scalars.  The two checks cover different faults: keep both for a file from somebody else.
+    ValueError names what failed: a truncated or over-long file, a count of 0 or above 2^32, the first rejected point
+    and why, or the failed consistency check.  A file that fails its format or point checks leaves the context
+    uninitialised; one that fails the consistency check leaves it initialised with no bases (the refused points are
+    dropped from the device)."""
+    size = os.path.getsize(path)
+    with open(path, "rb") as f:
+        head = f.read(8)
+    if len(head) < 8:
+        raise ValueError(f"truncated SRS file: {size} bytes")
+    n = struct.unpack("<Q", head)[0]
+    if n == 0 or n > 1 << 32:
+        raise ValueError(f"SRS file: a count of {n} points (1 .. 2^32 are accepted)")
+    want = 8 + 48 * n + 192
+    if size != want:
+        raise ValueError(f"{'truncated' if size < want else 'over-long'} SRS file: {size} bytes, {n} points need {want}")
+    g2 = np.fromfile(path, dtype=np.uint8, count=192, offset=8 + 48 * n)
+    h, beta_h = _g2_pair_from_bytes(ctx, g2.tobytes(), "the SRS file")
+    points = np.memmap(path, dtype=np.uint8, mode="r", offset=8, shape=(n, 48))
+    try:
+        ctx.init_compressed(points, domain_size, quot_domain_size, check_subgroup)
+    except DpError as e:
+        if e.code != DP_E_ARG or "rejected" not in e.msg:
+            raise
+        raise ValueError(f"SRS file: {e.msg.split(': ', 1)[1]}") from e
+    finally:
+        del points
+    key = OpenKey(G1_GEN, h, beta_h)
+    if check and not ctx.srs_check(np.frombuffer(g2_to_raw(h) + g2_to_raw(beta_h), dtype=np.uint8).reshape(2, 200)):
+        ctx.init(np.zeros((0, 104), dtype=np.uint8), domain_size, quot_domain_size)
+        raise ValueError("SRS file: the G1 points are not the consecutive powers g, tau g, tau^2 g, ... of the tau of (h, beta_h)")
+    return key

@@ -24,7 +24,7 @@ import time
 import numpy as np
 
 from ._binding import DP_E_ARG, FQ12_BYTES, DpError
-from .proof import Proof, g2_to_raw, point_from_raw, point_to_raw
+from .proof import Proof, VerifyingKey, g2_to_raw, point_from_raw, point_to_raw
 from .transcript import PlonkTranscript, R_MOD
 
 N_WIRES, N_QUOT, N_SIGMA_EVALS = 5, 5, 4
@@ -212,3 +212,13 @@ def batch_verify(ctx, open_key, items, timings: dict | None = None) -> bool:
         raise ValueError("batch_verify needs at least one proof")
     rs = [1 + secrets.randbelow(R_MOD - 1) for _ in items]
     return _check(ctx, open_key, items, rs, timings)
+
+
+def verify_bytes(ctx, vk_bytes, open_key_bytes, public_inputs, proof_bytes) -> bool:
+    """verify for a party that holds nothing but three byte strings - a verifying key (VerifyingKey.to_bytes), an open key
+    (OpenKey.to_bytes) and a proof (Proof.to_bytes) - and the public inputs: no tau, no SRS, no circuit, and a context that
+    was never initialised.  Every point is decoded and subgroup-checked on the GPU.  ValueError for a malformed encoding
+    or wrong shapes, False for a well-formed proof that is not accepted."""
+    from .srs import open_key_from_bytes
+    vk = VerifyingKey.from_bytes(ctx, vk_bytes)
+    return verify(ctx, vk, open_key_from_bytes(ctx, open_key_bytes), public_inputs, proof_from_bytes(ctx, proof_bytes))

@@ -45,7 +45,8 @@ extern "C" {
 #define DP_G1_COMPRESSED_BYTES 48 /* ark-serialize 0.3.0 compressed GroupAffine */
 #define DP_G1_PROJECTIVE_BYTES 144
 #define DP_G2_AFFINE_BYTES 200     /* raw ark 0.3 GroupAffine<g2::Parameters>: x.c0, x.c1, y.c0, y.c1, infinity, padding */
-#define DP_FQ12_BYTES 576          /* 12 Montgomery Fq in the order of the tower Fq2 -> Fq6 -> Fq12 (DESIGN.md 3.8)      */
+#define DP_G2_COMPRESSED_BYTES 96  /* ark-serialize 0.3 compressed GroupAffine<g2::Parameters>                            */
+#define DP_FQ12_BYTES 576         /* 12 Montgomery Fq in the order of the tower Fq2 -> Fq6 -> Fq12 (DESIGN.md 3.8)      */
 
 typedef struct dp_ctx dp_ctx;
 
@@ -107,6 +108,33 @@ int dp_srs_open_key(dp_ctx *ctx, const void *tau32, void *out400);
  * (DESIGN.md section 3.8).  A pair with a point at infinity contributes 1; k = 0 gives 1.  A G1 point off the curve,
  * a G2 point off the twist or outside the r-torsion, or a coordinate >= p is DP_E_ARG naming the first bad pair.   */
 int dp_multi_pairing(dp_ctx *ctx, const void *g1_104, const void *g2_200, size_t k, void *out576);
+
+/* ---- setup files (DESIGN.md section 3.9): the encodings an SRS, open-key or verifying-key file holds.  Only
+ * dp_get_bases_compressed and dp_srs_check need dp_init.  Buffers: host memory, or device memory of the context's GPU.
+ * The inverse of dp_g1_decompress: n raw G1Affine (104 B each, not validated; the identity flag is honoured) -> ark-serialize
+ * 0.3 compressed points (48 B each: canonical x little-endian, bit 7 of the last byte = (y > -y), bit 6 = identity).      */
+int dp_g1_compress(dp_ctx *ctx, const void *in104, size_t n, void *out48);
+/* bases [start, start + n) of an initialised context in that encoding, straight from the resident points               */
+int dp_get_bases_compressed(dp_ctx *ctx, uint64_t start, size_t n, void *out48);
+/* n raw G2Affine (200 B each) -> ark-serialize 0.3 compressed points (96 B each: canonical x.c0 then x.c1, 48 little-endian
+ * bytes each; bit 7 of the last byte = (y > -y) with Fq2 ordered by c1 first, then c0; bit 6 = identity).  n <= 2^20.    */
+int dp_g2_compress(dp_ctx *ctx, const void *in200, size_t n, void *out96);
+/* The inverse, with the reason codes of dp_g1_decompress: *why = 1 (a coordinate >= p), 2 (both flag bits), 3 (no such point
+ * on the twist y^2 = x^3 + 4 (u + 1)) or 4 (outside the r-torsion, checked when check_subgroup != 0).  A rejected point
+ * returns DP_E_ARG, writes nothing to out200 and sets *bad_index; on success *bad_index = n, *why = 0.  n <= 2^20.       */
+int dp_g2_decompress(dp_ctx *ctx, const void *in96, size_t n, int check_subgroup, void *out200, size_t *bad_index, int *why);
+/* Are the context's bases P_0 .. P_(N-1) the powers g, tau g, tau^2 g, ... of the tau of this open key?  g2_400 = h, beta h
+ * (two raw G2Affine, host).  *ok = 1 iff P_0 is the G1 generator and e(A, beta h) = e(B, h) for A = sum rho_i P_i and
+ * B = sum rho_i P_(i+1), i < N - 1, with 128-bit rho_i from ChaCha20 blocks (RFC 8439) keyed by seed32 (32 B; NULL: drawn
+ * from getrandom(2), DP_E_STATE if unavailable): an SRS that is not such a sequence passes with probability about 2^-128
+ * over the seed, so a seed the producer of the SRS could predict proves nothing.  Two MSMs over all N bases and one 2-pair
+ * pairing.  It does NOT replace the per-point subgroup check of dp_init_compressed: a component of a G1 point in the
+ * cofactor subgroup is invisible to the pairing.  A G2 point off the twist or outside the r-torsion is DP_E_ARG, as in
+ * dp_multi_pairing.  DP_E_STATE before dp_init or without bases; the context's state stays as it was.                    */
+int dp_srs_check(dp_ctx *ctx, const void *g2_400, const void *seed32, int *ok);
+/* the last dp_srs_check on ctx: host-clock ms of its scalar generation, its two MSMs and its pairing (each ends in a
+ * device synchronise; 0 for a phase that did not run), and A, B (2 x 144 B normalised G1Projective).  NULL = not wanted */
+int dp_last_srs_check(const dp_ctx *ctx, float *scalars_ms, float *msm_ms, float *pairing_ms, void *ab288);
 
 /* ---- PlonkSlave.varMsm (src/worker.rs:159-185) -----------------------------------------------
  * out = sum_{k < min(end-start, n_scalars)} scalars[k] * bases[start + k]
