@@ -26,6 +26,7 @@ EXPORTS = [
     "dp_srs_powers_of_tau",
     "dp_g1_decompress", "dp_msm_points", "dp_srs_open_key", "dp_multi_pairing",
     "dp_g1_compress", "dp_get_bases_compressed", "dp_g2_compress", "dp_g2_decompress", "dp_srs_check", "dp_last_srs_check",
+    "dp_srs_update", "dp_debug_srs_update_plain",
 ]
 
 
@@ -133,6 +134,8 @@ def bind(cdll: C.CDLL) -> C.CDLL:
         "dp_g2_decompress": (i, [vp, vp, sz, i, vp, C.POINTER(sz), C.POINTER(i)]),
         "dp_srs_check": (i, [vp, vp, vp, C.POINTER(i)]),
         "dp_last_srs_check": (i, [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), vp]),
+        "dp_srs_update": (i, [vp, vp, vp, vp, vp]),
+        "dp_debug_srs_update_plain": (i, [vp, vp, vp, vp, vp]),
         "dp_poly_eval": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_eval_dev": (i, [vp, vp, sz, vp, vp]),
         "dp_poly_lincomb": (i, [vp, C.POINTER(vp), C.POINTER(sz), vp, sz, vp, sz]),
@@ -693,6 +696,22 @@ class Context:
         ab = np.zeros((2, G1_PROJECTIVE_BYTES), dtype=np.uint8)
         self._ck(self.lib.dp_last_srs_check(self.h, C.byref(a), C.byref(b), C.byref(c), _addr(ab)))
         return {"scalars_ms": a.value, "msm_ms": b.value, "pairing_ms": c.value, "A": ab[0], "B": ab[1]}
+
+    def srs_update(self, g2_400, n: int, secret: int | None = None, out48=None, plain: bool = False):
+        """one ceremony contribution over the n resident bases (dp_srs_update): returns (the [n, 48] compressed points
+        s^i P_i, [2, 200] raw G2Affine s h, s beta h).  g2_400 = h, beta h.  secret None lets the library draw s; out48:
+        an [n, 48] uint8 array (a memory map of a file, say) or a device address to write the points to instead.  plain:
+        dp_debug_srs_update_plain, the reference method"""
+        q = np.ascontiguousarray(g2_400, dtype=np.uint8).reshape(2, G2_AFFINE_BYTES)
+        g2 = np.zeros((2, G2_AFFINE_BYTES), dtype=np.uint8)
+        if out48 is None:
+            out48 = np.zeros((n, G1_COMPRESSED_BYTES), dtype=np.uint8)
+        elif not isinstance(out48, int):
+            assert out48.dtype == np.uint8 and out48.size == n * G1_COMPRESSED_BYTES and out48.flags["C_CONTIGUOUS"]
+        s = self._tau_bytes(secret) if secret is not None else None
+        f = self.lib.dp_debug_srs_update_plain if plain else self.lib.dp_srs_update
+        self._ck(f(self.h, s, _addr(q), _addr(out48), _addr(g2)))
+        return out48, g2
 
     def init_ptr(self, bases_ptr: int, n_bases: int, domain_size: int, quot_domain_size: int):
         """PlonkSlave.init with the raw GroupAffine array at `bases_ptr` (host or device memory)"""

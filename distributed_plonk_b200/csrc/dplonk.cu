@@ -2680,6 +2680,21 @@ int dp_debug_gen_bases(dp_ctx *ctx, uint64_t seed, size_t n, void *out) {
     return DP_OK;
 }
 
+// tau^i = A[i mod 2^h] * B[i >> h] for i < n: A[a] = tau^a, B[b] = tau^(2^h b), about sqrt(n) host products each
+// (Montgomery form; h >= min_log_a).  Returns h.
+static uint32_t srs_power_tables(const Fr &tau, uint64_t n, uint32_t min_log_a, std::vector<Fr> &pow_a, std::vector<Fr> &pow_b) {
+    uint32_t log_a = (log2_ceil_u64(n) + 1) / 2;
+    if (log_a < min_log_a) log_a = min_log_a;
+    const uint64_t n_a = (uint64_t)1 << log_a, n_b = (n + n_a - 1) >> log_a;
+    pow_a.assign(n_a, Fr::one());
+    pow_b.assign(n_b, Fr::one());
+    const Fr t = tau.to_mont();
+    for (uint64_t a = 1; a < n_a; a++) pow_a[a] = pow_a[a - 1] * t;
+    const Fr step = pow_a[n_a - 1] * t;
+    for (uint64_t b = 1; b < n_b; b++) pow_b[b] = pow_b[b - 1] * step;
+    return log_a;
+}
+
 int dp_srs_powers_of_tau(dp_ctx *ctx, const void *tau32, size_t n, void *out104) {
     if (!ctx) return fail(ctx, DP_E_ARG, "dp_srs_powers_of_tau: ctx is NULL");
     if (n && (!tau32 || !out104)) return fail(ctx, DP_E_ARG, "dp_srs_powers_of_tau: NULL argument");
@@ -2690,16 +2705,9 @@ int dp_srs_powers_of_tau(dp_ctx *ctx, const void *tau32, size_t n, void *out104)
     if (tau.is_zero()) return fail(ctx, DP_E_ARG, "dp_srs_powers_of_tau: tau is zero");
     if (!tau.canon_is_reduced()) return fail(ctx, DP_E_ARG, "dp_srs_powers_of_tau: tau is not a canonical scalar (tau >= r)");
     DP_CUDA(ctx, cudaSetDevice(ctx->device));
-    // tau^i = A[i mod 2^h] * B[i >> h]: A[a] = tau^a, B[b] = tau^(2^h b), about sqrt(n) host products each
-    const uint32_t log_a = (log2_ceil_u64(n) + 1) / 2;
-    const uint64_t n_a = (uint64_t)1 << log_a, n_b = (n + n_a - 1) >> log_a;
-    std::vector<Fr> pow_a(n_a), pow_b(n_b);
-    const Fr t = tau.to_mont();
-    pow_a[0] = Fr::one();
-    for (uint64_t a = 1; a < n_a; a++) pow_a[a] = pow_a[a - 1] * t;
-    const Fr step = pow_a[n_a - 1] * t;
-    pow_b[0] = Fr::one();
-    for (uint64_t b = 1; b < n_b; b++) pow_b[b] = pow_b[b - 1] * step;
+    std::vector<Fr> pow_a, pow_b;
+    const uint32_t log_a = srs_power_tables(tau, n, 0, pow_a, pow_b);
+    const uint64_t n_a = pow_a.size(), n_b = pow_b.size();
     call_begin(ctx);
     Scratch tmp(ctx->pool);
     Fr *da = tmp.get<Fr>(n_a), *db = tmp.get<Fr>(n_b);
@@ -3032,6 +3040,102 @@ int dp_srs_check(dp_ctx *ctx, const void *g2_400, const void *seed32, int *ok) {
     ctx->srs_check_ms[2] = ms_since(t0);
     *ok = memcmp(e, one, sizeof e) == 0 ? 1 : 0;
     return DP_OK;
+}
+
+// ---- ceremony: one contribution Q_i = s^i P_i over the resident bases, and s h, s beta h (DESIGN.md section 3.10)
+static int srs_update(dp_ctx *ctx, const void *s32, const void *g2_400, void *out48, void *out400, bool glv, const char *who) {
+    if (!ctx) return fail(ctx, DP_E_ARG, "%s: ctx is NULL", who);
+    if (!g2_400 || !out48 || !out400) return fail(ctx, DP_E_ARG, "%s: NULL argument", who);
+    if (!ctx->inited) return fail(ctx, DP_E_STATE, "%s before dp_init", who);
+    const uint64_t n = ctx->n_bases;
+    if (n == 0) return fail(ctx, DP_E_STATE, "%s: the context holds no bases", who);
+    // the secret and everything derived from it on the host: wiped on every return
+    Fr s = Fr::zero();
+    std::vector<Fr> pow_a, pow_b;
+    struct HostWipe {
+        Fr &s;
+        std::vector<Fr> &a, &b;
+        ~HostWipe() {
+            explicit_bzero((void *)&s, sizeof s);
+            if (!a.empty()) explicit_bzero((void *)a.data(), a.size() * sizeof(Fr));
+            if (!b.empty()) explicit_bzero((void *)b.data(), b.size() * sizeof(Fr));
+        }
+    } host_wipe{s, pow_a, pow_b};
+    if (s32) {
+        memcpy(s.l, s32, sizeof s.l);
+        if (s.is_zero()) return fail(ctx, DP_E_ARG, "%s: s is zero", who);
+        if (!s.canon_is_reduced()) return fail(ctx, DP_E_ARG, "%s: s is not a canonical scalar (s >= r)", who);
+    } else {
+        while (s.is_zero() || !s.canon_is_reduced()) {  // uniform in 1 .. r - 1: r > 2^254, so 255 random bits hit it often
+            size_t got = 0;
+            while (got < sizeof s.l) {
+                const ssize_t r = getrandom(reinterpret_cast<uint8_t *>(s.l) + got, sizeof s.l - got, 0);
+                if (r < 0) return fail(ctx, DP_E_STATE, "%s: getrandom failed; pass s", who);
+                got += (size_t)r;
+            }
+            s.l[7] &= 0x7fffffffu;
+        }
+    }
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    const uint32_t log_a = srs_power_tables(s, n, 1, pow_a, pow_b);  // h >= 1: pow_a[1] = s for the G2 kernel
+    const uint64_t n_a = pow_a.size(), n_b = pow_b.size();
+    call_begin(ctx);
+    Scratch tmp(ctx->pool);
+    Fr *da = tmp.get<Fr>(n_a), *db = tmp.get<Fr>(n_b);
+    const uint64_t chunk = n < SRS_CHUNK ? n : SRS_CHUNK;
+    uint32_t *staging = tmp.get<uint32_t>(chunk * 12);
+    uint64_t *g2_in = tmp.get<uint64_t>(2 * 25), *g2_out = tmp.get<uint64_t>(2 * 25);
+    unsigned long long *bad = tmp.get<unsigned long long>(1), verdict = ~0ull;
+    // the pool hands its blocks out again (DESIGN.md section 3.5): the power tables are zeroed, in stream order, before
+    // Scratch returns them, on every path
+    struct DeviceWipe {
+        dp_ctx *ctx;
+        Fr *a, *b;
+        uint64_t n_a, n_b;
+        ~DeviceWipe() {
+            if (a) cudaMemsetAsync(a, 0, n_a * sizeof(Fr), ctx->stream);
+            if (b) cudaMemsetAsync(b, 0, n_b * sizeof(Fr), ctx->stream);
+            cudaStreamSynchronize(ctx->stream);
+        }
+    } device_wipe{ctx, da, db, n_a, n_b};
+    if (!da || !db || !staging || !g2_in || !g2_out || !bad) return fail(ctx, DP_E_OOM, "%s buffers", who);
+    DP_CUDA(ctx, cudaMemcpyAsync(da, pow_a.data(), n_a * sizeof(Fr), cudaMemcpyHostToDevice, ctx->stream));
+    DP_CUDA(ctx, cudaMemcpyAsync(db, pow_b.data(), n_b * sizeof(Fr), cudaMemcpyHostToDevice, ctx->stream));
+    DP_CUDA(ctx, cudaMemcpyAsync(g2_in, g2_400, 2 * (size_t)DP_G2_AFFINE_BYTES, cudaMemcpyDefault, ctx->stream));
+    DP_CUDA(ctx, cudaMemcpyAsync(bad, &verdict, sizeof verdict, cudaMemcpyHostToDevice, ctx->stream));
+    DP_LAUNCH(srs_update_g2_kernel, dim3(1), dim3(32), 0, ctx->stream, (const Fr *)da, (const uint64_t *)g2_in, g2_out, bad);
+    ctx->launches++;
+    DP_CUDA(ctx, cudaMemcpyAsync(&verdict, bad, sizeof verdict, cudaMemcpyDeviceToHost, ctx->stream));
+    DP_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // a rejected G2 point is refused before the bulk work
+    if (verdict != ~0ull) {
+        static const char *const reason[] = {"", "", "", "a coordinate is not below p", "the point is not on the twist",
+                                             "the point is not in the r-torsion subgroup"};
+        return fail(ctx, DP_E_ARG, "%s: %s rejected: %s", who, (verdict >> 8) == 1 ? "h" : "beta h", reason[(verdict & 0xff) < 6 ? verdict & 0xff : 0]);
+    }
+    const Fq beta = glv_beta();
+    for (uint64_t first = 0; first < n; first += chunk) {
+        const uint64_t end = first + chunk < n ? first + chunk : n;
+        if (glv)
+            DP_LAUNCH(srs_update_kernel<true>, dim3(blocks_for(end - first, AFF_TPB)), dim3(AFF_TPB), 0, ctx->stream, (const G1Affine *)ctx->bases,
+                      (const Fr *)da, (const Fr *)db, log_a, first, end, beta, staging);
+        else
+            DP_LAUNCH(srs_update_kernel<false>, dim3(blocks_for(end - first, AFF_TPB)), dim3(AFF_TPB), 0, ctx->stream, (const G1Affine *)ctx->bases,
+                      (const Fr *)da, (const Fr *)db, log_a, first, end, beta, staging);
+        ctx->launches++;
+        DP_CUDA(ctx, cudaGetLastError());
+        DP_CUDA(ctx, cudaMemcpyAsync((uint8_t *)out48 + first * DP_G1_COMPRESSED_BYTES, staging, (end - first) * DP_G1_COMPRESSED_BYTES,
+                                     cudaMemcpyDefault, ctx->stream));  // host or device memory
+    }
+    DP_CUDA(ctx, cudaMemcpyAsync(out400, g2_out, 2 * (size_t)DP_G2_AFFINE_BYTES, cudaMemcpyDefault, ctx->stream));
+    return call_end(ctx, true);
+}
+
+int dp_srs_update(dp_ctx *ctx, const void *s32, const void *g2_400, void *out48, void *out400) {
+    return srs_update(ctx, s32, g2_400, out48, out400, true, "dp_srs_update");
+}
+
+int dp_debug_srs_update_plain(dp_ctx *ctx, const void *s32, const void *g2_400, void *out48, void *out400) {
+    return srs_update(ctx, s32, g2_400, out48, out400, false, "dp_debug_srs_update_plain");
 }
 
 int dp_last_srs_check(const dp_ctx *ctx, float *scalars_ms, float *msm_ms, float *pairing_ms, void *ab288) {

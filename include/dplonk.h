@@ -136,6 +136,17 @@ int dp_srs_check(dp_ctx *ctx, const void *g2_400, const void *seed32, int *ok);
  * device synchronise; 0 for a phase that did not run), and A, B (2 x 144 B normalised G1Projective).  NULL = not wanted */
 int dp_last_srs_check(const dp_ctx *ctx, float *scalars_ms, float *msm_ms, float *pairing_ms, void *ab288);
 
+/* ---- setup ceremony (DESIGN.md section 3.10): one contribution to a powers-of-tau SRS.  For the N resident bases P_i of
+ * an initialised context and g2_400 = h, beta h (two raw G2Affine): out48[i] = s^i P_i as 48-byte compressed points
+ * (the encoding of dp_g1_compress), and out400 = s h, s beta h (two raw G2Affine).  If P_i = tau^i g and beta h = tau h,
+ * the output is the SRS of tau s.  s32: 32 B canonical, 0 < s < r, else DP_E_ARG; NULL draws s from getrandom(2)
+ * (DP_E_STATE if unavailable).  s lives only inside the call: its host copies and the device power tables are zeroed
+ * before it returns.  A G2 input off the twist, outside the r-torsion or with a coordinate >= p is DP_E_ARG, before any
+ * G1 work.  The bases must lie in the r-torsion (dp_init_compressed with check_subgroup guarantees it).  out48, out400:
+ * host memory or device memory of the context's GPU.  DP_E_STATE before dp_init or without bases; the context's state
+ * (bases, MSM tables and tuning) stays as it was.                                                                        */
+int dp_srs_update(dp_ctx *ctx, const void *s32, const void *g2_400, void *out48, void *out400);
+
 /* ---- PlonkSlave.varMsm (src/worker.rs:159-185) -----------------------------------------------
  * out = sum_{k < min(end-start, n_scalars)} scalars[k] * bases[start + k]
  * (VariableBaseMSM::multi_scalar_mul(&bases[start..end], &scalars) truncates to the shorter).
@@ -410,6 +421,10 @@ int dp_msm_tuning_all(const dp_ctx *ctx, float ms_by_levels[4]);
  * computed on the device and written to `out` (host memory, or device memory of the same GPU); feeds
  * dp_init in benches and tests */
 int dp_debug_gen_bases(dp_ctx *ctx, uint64_t seed, size_t n, void *out);
+
+/* dp_srs_update computed with the plain 255-bit double-and-add per point instead of the endomorphism split: the same
+ * bytes, slower; the reference dp_srs_update is measured and tested against                                   */
+int dp_debug_srs_update_plain(dp_ctx *ctx, const void *s32, const void *g2_400, void *out48, void *out400);
 
 /* test hook: lower the pass-planning limits (sub-transform sizes 2^k handled by one kernel pass;
  * defaults 11 / 9) and/or steer the MSM (0 = automatic: precomputed window multiples when the SRS is

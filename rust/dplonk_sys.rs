@@ -55,6 +55,7 @@ extern "C" {
     pub fn dp_msm_points(ctx: *mut dp_ctx, points104: *const u8, scalars32: *const u8, n: usize, out144: *mut u8) -> c_int;
     pub fn dp_srs_open_key(ctx: *mut dp_ctx, tau32: *const u8, out400: *mut u8) -> c_int;
     pub fn dp_multi_pairing(ctx: *mut dp_ctx, g1_104: *const u8, g2_200: *const u8, k: usize, out576: *mut u8) -> c_int;
+    pub fn dp_srs_update(ctx: *mut dp_ctx, s32: *const u8, g2_400: *const u8, out48: *mut c_void, out400: *mut c_void) -> c_int;
     pub fn dp_msm(ctx: *mut dp_ctx, start: u64, end: u64, scalars: *const u8, n_scalars: usize, out144: *mut u8) -> c_int;
     pub fn dp_msm_submit(ctx: *mut dp_ctx, id: u64, start: u64, end: u64, scalars: *const u8, n_scalars: usize) -> c_int;
     pub fn dp_msm_collect(ctx: *mut dp_ctx, id: u64, out144: *mut u8) -> c_int;
