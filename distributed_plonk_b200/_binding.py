@@ -9,6 +9,8 @@ DP_OK, DP_E_ARG, DP_E_STATE, DP_E_OOM, DP_E_CUDA, DP_E_COMM = 0, -1, -2, -3, -4,
 FR_BYTES, G1_AFFINE_BYTES, G1_PROJECTIVE_BYTES = 32, 104, 144
 G1_COMPRESSED_BYTES, G2_AFFINE_BYTES, FQ12_BYTES = 48, 200, 576
 G2_COMPRESSED_BYTES = 96
+LINCOMB_MAX = 32                 # operands of one dp_poly_lincomb call (RND_MAX_POLYS)
+FR_MODULUS = 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFFFFF00000001
 
 EXPORTS = [
     "dp_create", "dp_destroy", "dp_last_error", "dp_version", "dp_init", "dp_msm", "dp_commit", "dp_fft_init",
@@ -27,6 +29,7 @@ EXPORTS = [
     "dp_g1_decompress", "dp_msm_points", "dp_srs_open_key", "dp_multi_pairing",
     "dp_g1_compress", "dp_get_bases_compressed", "dp_g2_compress", "dp_g2_decompress", "dp_srs_check", "dp_last_srs_check",
     "dp_srs_update", "dp_debug_srs_update_plain",
+    "dp_quotient_evals_acc_dev", "dp_quotient_evals_slice_acc_dev",
 ]
 
 
@@ -117,6 +120,8 @@ def bind(cdll: C.CDLL) -> C.CDLL:
         "dp_ntt_dev_quot_slice": (i, [vp, vp, sz, u32, vp, i]),
         "dp_quotient_evals_tail_dev": (i, [vp, C.POINTER(QuotientArgs), C.POINTER(QuotientTails), vp]),
         "dp_quotient_evals_slice_tail_dev": (i, [vp, C.POINTER(QuotientArgs), C.POINTER(QuotientTails), u32, vp]),
+        "dp_quotient_evals_acc_dev": (i, [vp, C.POINTER(QuotientArgs), C.POINTER(QuotientTails), vp, vp]),
+        "dp_quotient_evals_slice_acc_dev": (i, [vp, C.POINTER(QuotientArgs), C.POINTER(QuotientTails), u32, vp, vp]),
         "dp_poly_blind_dev": (i, [vp, vp, sz, u32, vp]),
         "dp_wire_permutation_scratch_bytes": (i, [sz, sz, u64, C.POINTER(sz)]),
         "dp_wire_permutation_dev": (i, [vp, vp, sz, sz, u64, vp, sz, vp]),
@@ -397,6 +402,19 @@ class Context:
         t = self._quotient_tails(tails)
         self._ck(self.lib.dp_quotient_evals_slice_tail_dev(self.h, C.byref(q), C.byref(t), slice_, out_ptr))
 
+    def quotient_evals_acc_dev(self, selectors, sigmas, wires, perm, pub_input, k, alpha, beta, gamma, tails, scale, out_ptr: int,
+                               slice_: int | None = None):
+        """out[pt] += scale * quotient(pt) (a batch proof's round 3): over the whole coset (slice_ None, arrays of m points)
+        or over slice slice_ (arrays of n points); tails as in quotient_evals_tail_dev, or None (unblinded); scale raw Fr"""
+        keep = []
+        q = self._quotient_args(selectors, sigmas, wires, perm, pub_input, k, alpha, beta, gamma, keep)
+        t = C.byref(self._quotient_tails(tails)) if tails is not None else None
+        sc = np.ascontiguousarray(scale, dtype=np.uint64)
+        if slice_ is None:
+            self._ck(self.lib.dp_quotient_evals_acc_dev(self.h, C.byref(q), t, _addr(sc), out_ptr))
+        else:
+            self._ck(self.lib.dp_quotient_evals_slice_acc_dev(self.h, C.byref(q), t, slice_, _addr(sc), out_ptr))
+
     def poly_blind_dev(self, coeffs_ptr: int, n: int, k: int, blind: np.ndarray | None = None):
         """coeffs += b(X) * (X^n - 1) in place (n + k Fr on the device); blind = [k,4] raw Fr, or None: the library draws
         the k scalars from the OS entropy pool and they never leave it"""
@@ -457,8 +475,17 @@ class Context:
         cf = np.ascontiguousarray(coeffs, dtype=np.uint64)
         k = len(polys)
         if out_ptr is not None:
-            ptrs, ln = (C.c_void_p * k)(*polys), (C.c_size_t * k)(*lens)
-            self._ck(self.lib.dp_poly_lincomb_dev(self.h, ptrs, ln, _addr(cf), k, out_ptr, out_len))
+            # more than LINCOMB_MAX operands: the output accumulates in place, [out] + the next 31 with coefficient 1
+            head = min(k, LINCOMB_MAX)
+            ptrs, ln = (C.c_void_p * head)(*polys[:head]), (C.c_size_t * head)(*lens[:head])
+            self._ck(self.lib.dp_poly_lincomb_dev(self.h, ptrs, ln, _addr(np.ascontiguousarray(cf[:head])), head, out_ptr, out_len))
+            one = np.frombuffer(((1 << 256) % FR_MODULUS).to_bytes(32, "little"), dtype=np.uint64)
+            for s in range(head, k, LINCOMB_MAX - 1):
+                e = min(k, s + LINCOMB_MAX - 1)
+                ptrs = (C.c_void_p * (1 + e - s))(out_ptr, *polys[s:e])
+                ln = (C.c_size_t * (1 + e - s))(out_len, *lens[s:e])
+                c2 = np.ascontiguousarray(np.concatenate([one[None], cf[s:e]]))
+                self._ck(self.lib.dp_poly_lincomb_dev(self.h, ptrs, ln, _addr(c2), 1 + e - s, out_ptr, out_len))
             return None
         ps = [np.ascontiguousarray(x, dtype=np.uint64) for x in polys]
         ln = [x.shape[0] for x in ps]

@@ -3349,8 +3349,9 @@ int poly_suffix_device(dp_ctx *ctx, const Fr *in, uint64_t n, const Fr *pw, uint
 // points g * omega_m^(k + (m/n) i), written to out_dev[k + (m/n) i]
 // tails (checked by quotient_tails_check, not all empty): the wires and z have more than n coefficients, the arrays hold the
 // evaluations of their first n (QuotientTailArgs)
+// scale (accumulating form, QuotientAcc): out_dev[pt] += scale * quotient(pt) instead of out_dev[pt] = quotient(pt)
 int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arrays /* 25 device arrays */, Fr *out_dev,
-                    int slice = -1, const dp_quotient_tails *tails = nullptr) {
+                    int slice = -1, const dp_quotient_tails *tails = nullptr, const Fr *scale = nullptr) {
     const DomainDev &dq = ctx->dom[1], &dg = ctx->dom[0];
     const uint64_t m = dq.n(), n = dg.n();
     if (m < n || m / n > RND_MAX_RATIO) return fail(ctx, DP_E_ARG, "quotient domain / gate domain = %llu, supported: 1..%d", (unsigned long long)(m / n), RND_MAX_RATIO);
@@ -3381,6 +3382,10 @@ int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arr
     }
     for (uint32_t i = q.ratio; i < RND_MAX_RATIO; i++) q.zh_inv[i] = Fr::zero();
     if (slice >= (int)q.ratio) return fail(ctx, DP_E_ARG, "quotient slice %d of %u", slice, q.ratio);
+    if (scale) {   // scale * (zh_inv (gate + alpha perm) + alpha^2/n (z - 1)/(x - 1)): both products take the scale
+        for (uint32_t i = 0; i < q.ratio; i++) q.zh_inv[i] = q.zh_inv[i] * *scale;
+        q.alpha_sq_div_n = q.alpha_sq_div_n * *scale;
+    }
     q.H = dq.H;
     q.m = m;
     q.log_m = dq.log_n;
@@ -3439,7 +3444,12 @@ int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arr
         DP_CUDA(ctx, cudaGetLastError());
         return DP_OK;
     };
-    if (!tails) return launch(q);
+    if (!tails) {
+        if (!scale) return launch(q);
+        QuotientAcc<QuotientArgs> qa;
+        static_cast<QuotientArgs &>(qa) = q;
+        return launch(qa);
+    }
     QuotientTailArgs qt;
     static_cast<QuotientArgs &>(qt) = q;
     for (int j = 0; j < 5; j++) {
@@ -3450,7 +3460,10 @@ int quotient_device(dp_ctx *ctx, const dp_quotient_args &a, const Fr *const *arr
     qt.z_tail_len = (uint32_t)tails->perm_len;
     for (uint32_t i = 0; i < RND_MAX_RATIO; i++) qt.xn[i] = i < q.ratio ? xn[i] : Fr::zero();
     qt.omega_n = fr_domain_gen(dg.log_n);
-    return launch(qt);
+    if (!scale) return launch(qt);
+    QuotientAcc<QuotientTailArgs> qta;
+    static_cast<QuotientTailArgs &>(qta) = qt;
+    return launch(qta);
 }
 
 const void *const *quotient_ptrs(const dp_quotient_args &a, const void *flat[25]) {
@@ -3566,6 +3579,43 @@ int dp_quotient_evals_slice_tail_dev(dp_ctx *ctx, const dp_quotient_args *slice_
                                      void *out_dev) {
     if (!tails) return fail(ctx, DP_E_ARG, "dp_quotient_evals_slice_tail_dev: NULL tails");
     return quotient_slice_any(ctx, slice_arrays, tails, slice, out_dev, "dp_quotient_evals_slice_tail_dev");
+}
+
+// the accumulating entries: slice < 0 = the whole coset (25 arrays of m points), else one slice (25 arrays of n points)
+static int quotient_acc_any(dp_ctx *ctx, const dp_quotient_args *arrays, const dp_quotient_tails *tails, int slice, const void *scale32,
+                            void *out_dev, const char *who) {
+    DP_TRY(quotient_check(ctx, arrays, out_dev, who));
+    if (!scale32) return fail(ctx, DP_E_ARG, "%s: NULL scale", who);
+    Fr scale;
+    memcpy(&scale, scale32, sizeof scale);
+    if (!scale.canon_is_reduced()) return fail(ctx, DP_E_ARG, "%s: the scale is not below r", who);
+    bool any = false;
+    if (tails) DP_TRY(quotient_tails_check(ctx, tails, out_dev, &any, who));
+    const DomainDev &dg = ctx->dom[0], &dq = ctx->dom[1];
+    const uint64_t n = dg.n(), m = dq.n();
+    if (slice >= 0 && (m < n || (uint64_t)slice >= m / n))
+        return fail(ctx, DP_E_ARG, "%s: slice %d of %llu", who, slice, (unsigned long long)(m < n ? 0 : m / n));
+    const uint64_t in_len = slice < 0 ? m : n;
+    const void *flat[25];
+    quotient_ptrs(*arrays, flat);
+    for (int i = 0; i < 25; i++)   // the output is read as well as written: no input may share its memory
+        if (ranges_overlap(flat[i], in_len * sizeof(Fr), out_dev, m * sizeof(Fr)))
+            return fail(ctx, DP_E_ARG, "%s: the output overlaps input %d", who, i);
+    DP_CUDA(ctx, cudaSetDevice(ctx->device));
+    call_begin(ctx);
+    DP_TRY(quotient_device(ctx, *arrays, reinterpret_cast<const Fr *const *>(flat), (Fr *)out_dev, slice, any ? tails : nullptr, &scale));
+    return call_end(ctx, true);
+}
+
+int dp_quotient_evals_acc_dev(dp_ctx *ctx, const dp_quotient_args *dev_arrays, const dp_quotient_tails *tails, const void *scale32,
+                              void *out_dev) {
+    return quotient_acc_any(ctx, dev_arrays, tails, -1, scale32, out_dev, "dp_quotient_evals_acc_dev");
+}
+
+int dp_quotient_evals_slice_acc_dev(dp_ctx *ctx, const dp_quotient_args *slice_arrays, const dp_quotient_tails *tails, uint32_t slice,
+                                    const void *scale32, void *out_dev) {
+    if (slice > (uint32_t)RND_MAX_RATIO) return fail(ctx, DP_E_ARG, "dp_quotient_evals_slice_acc_dev: slice %u", slice);
+    return quotient_acc_any(ctx, slice_arrays, tails, (int)slice, scale32, out_dev, "dp_quotient_evals_slice_acc_dev");
 }
 
 static int poly_eval_any(dp_ctx *ctx, const void *coeffs, size_t n, const void *point, void *out32, bool on_device, const char *who) {

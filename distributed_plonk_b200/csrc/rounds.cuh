@@ -167,9 +167,16 @@ DP_D Fr quotient_tail_at(const Fr *t, uint32_t len, const Fr &y) {
     return acc;
 }
 
+// Accumulating form (batch proofs, DESIGN.md 3.11): out[pt] += scale * quotient(pt).  The host folds the scale into zh_inv[]
+// and alpha_sq_div_n, so the kernel's extra work is one load and one addition.  A distinct argument type rather than a
+// template flag, so the plain and tail instantiations keep their names and their code.
+template <typename Base>
+struct QuotientAcc : Base {};
+
 template <bool TABLE, typename Args = QuotientArgs>
 __global__ void __launch_bounds__(QUO_TPB) quotient_kernel(Args q) {
-    constexpr bool TAIL = std::is_same<Args, QuotientTailArgs>::value;
+    constexpr bool TAIL = std::is_base_of<QuotientTailArgs, Args>::value;
+    constexpr bool ACC = std::is_same<Args, QuotientAcc<QuotientArgs>>::value || std::is_same<Args, QuotientAcc<QuotientTailArgs>>::value;
     const uint64_t i = (uint64_t)blockIdx.x * QUO_TPB + threadIdx.x;
     const bool live = i < q.pts;
     const uint64_t pt = q.first + (uint64_t)q.step * i;  // the point's index in the quotient coset
@@ -225,6 +232,7 @@ __global__ void __launch_bounds__(QUO_TPB) quotient_kernel(Args q) {
     Fr r = qmul(q.zh_inv[pt % q.ratio], gate + qmul(q.alpha, acc1 - acc2));
     // (z - 1) L_1 alpha^2 / Z_H = alpha^2/n (z - 1) / (x - 1)   (lines 493-499)
     r = r + qmul(qmul(q.alpha_sq_div_n, zi - one), inv_xm1);
+    if constexpr (ACC) r = r + gmem_ld(q.out + pt);
     gmem_st(q.out + pt, r);
 }
 

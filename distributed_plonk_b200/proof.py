@@ -221,3 +221,60 @@ class Proof:
         return (vec(self.wires_poly_comms, g1_compress) + g1_compress(self.prod_perm_poly_comm) + vec(self.split_quot_poly_comms, g1_compress)
                 + g1_compress(self.opening_proof) + g1_compress(self.shifted_opening_proof)
                 + vec(self.wires_evals, fr) + vec(self.wire_sigma_evals, fr) + fr(self.perm_next_eval))
+
+
+@dataclass
+class ProofEvaluations:
+    """one instance's evaluations in a BatchProof: 5 wires and 4 sigmas at zeta, z at zeta * omega (canonical ints)"""
+    wires_evals: list
+    wire_sigma_evals: list
+    perm_next_eval: int
+
+    def evaluations(self) -> list:
+        return list(self.wires_evals) + list(self.wire_sigma_evals) + [self.perm_next_eval]
+
+
+@dataclass
+class BatchProof:
+    """k instances of one circuit proved together (ResidentProver.prove_batch, DESIGN.md 3.11): per instance its 5 wire
+    commitments, its permutation-product commitment and its evaluations; shared, the 5 quotient-chunk commitments of the
+    folded quotient and the two opening proofs.  Points affine (x, y) or None, evaluations canonical ints."""
+    wires_poly_comms_vec: list
+    prod_perm_poly_comms_vec: list
+    poly_evals_vec: list
+    split_quot_poly_comms: list
+    opening_proof: tuple | None
+    shifted_opening_proof: tuple | None
+
+    def __len__(self) -> int:
+        return len(self.wires_poly_comms_vec)
+
+    @classmethod
+    def from_raw(cls, k: int, commitments, evals) -> "BatchProof":
+        """from what the batch rounds return: 6k + 7 commitments (144 B: 5k wires, k z, 5 quotient chunks, the two opening
+        proofs) and 10k evaluations (raw Fr: per instance 5 wires, 4 sigmas, z at zeta * omega)"""
+        p = [point_from_jacobian(c) for c in commitments]
+        e = [fr_to_int(v) for v in evals]
+        assert len(p) == 6 * k + 7 and len(e) == 10 * k
+        q = 6 * k
+        return cls([p[5 * i:5 * i + 5] for i in range(k)], p[5 * k:6 * k],
+                   [ProofEvaluations(e[10 * i:10 * i + 5], e[10 * i + 5:10 * i + 9], e[10 * i + 9]) for i in range(k)],
+                   p[q:q + 5], p[q + 5], p[q + 6])
+
+    def instance(self, i: int) -> Proof:
+        """instance i's share as a Proof, with the shared quotient and openings (a batch of one is exactly that Proof)"""
+        e = self.poly_evals_vec[i]
+        return Proof(list(self.wires_poly_comms_vec[i]), self.prod_perm_poly_comms_vec[i], list(self.split_quot_poly_comms),
+                     self.opening_proof, self.shifted_opening_proof, list(e.wires_evals), list(e.wire_sigma_evals), e.perm_next_eval)
+
+    def to_bytes(self) -> bytes:
+        """ark-serialize 0.3 conventions, as Proof.to_bytes: wires_poly_comms_vec (Vec of Vecs of 5 points),
+        prod_perm_poly_comms_vec, poly_evals_vec (Vec of records: Vec of 5 wire evals, Vec of 4 sigma evals, perm_next_eval),
+        split_quot_poly_comms, opening_proof, shifted_opening_proof.  368 + 632 k bytes.  This library's own record: byte
+        parity with jf-plonk's BatchProof is not claimed."""
+        vec = lambda items, enc: struct.pack("<Q", len(items)) + b"".join(enc(x) for x in items)
+        fr = lambda v: int(v).to_bytes(32, "little")
+        ev = lambda e: vec(e.wires_evals, fr) + vec(e.wire_sigma_evals, fr) + fr(e.perm_next_eval)
+        return (vec(self.wires_poly_comms_vec, lambda ws: vec(ws, g1_compress)) + vec(self.prod_perm_poly_comms_vec, g1_compress)
+                + vec(self.poly_evals_vec, ev) + vec(self.split_quot_poly_comms, g1_compress)
+                + g1_compress(self.opening_proof) + g1_compress(self.shifted_opening_proof))

@@ -26,6 +26,8 @@ what the reference's FakeStandardTranscript feeds it, dispatcher2.rs:44-154) of 
 each round's commitments and evaluations, so it returns a Proof (proof.py) that a PLONK verifier accepts; blinded by
 default.  The hashing is host work on a few kilobytes; the verifying-key prefix is hashed once per load_circuit.
 prove and prove_witness still take the challenges as inputs (tests, benchmarks), and make the same library calls.
+prove_batch proves k witnesses of the loaded circuit with one transcript, one quotient sum_i alpha^(3i) Q_i and one pair of
+openings (DESIGN.md 3.11); every path runs the same per-round helpers over a list of instances.
 The proving key (13 selector + 5 sigma polynomials in coefficient form, sigma / identity permutation
 evaluations) stays resident across proofs, as `State` keeps the bases (worker.rs:42-59).
 
@@ -54,6 +56,8 @@ class ResidentProver:
     # with WHOLE_MARGIN_M quotient-domain buffers (the final iNTT(8n)'s scratch) and WHOLE_MARGIN_BYTES to spare, "sliced"
     # otherwise.  (The cached 1/(x - 1) table of m points is optional: the quotient falls back to its tree variant without it.)
     WHOLE_MARGIN_M, WHOLE_MARGIN_BYTES = 1, 1 << 30
+    # prove_batch: device memory left free beside the batch's instances (MSM and quotient scratch), and the emulator's cap
+    BATCH_MARGIN_BYTES, CPU_MAX_BATCH = 1 << 30, 64
 
     def __init__(self, ctx, torch, log_n: int, device: str, field, quotient: str = "auto"):
         """field: helpers over raw Montgomery Fr as np.uint64[4] - mul(a,b), add(a,b), sub(a,b), inv(a), from_u64(v),
@@ -90,6 +94,8 @@ class ResidentProver:
         # slice buffers are the heads of the whole-domain ones): tools/bench_resident.py times both modes on one prover that way.
         self.big = [buf(m) for _ in range(N_COEF)] if quotient == "whole" else None
         self.slices = [t[:n] for t in self.big] if self.big is not None else [buf(n) for _ in range(N_COEF)]
+        self._own = _Instance(self.wire_eval, self.pub, self.wire_coef, self.z)   # a single proof's instance, instance 0 of a batch
+        self._extra = []                                       # prove_batch: instances 1, 2, ... (kept for the next batch)
         self._srs_checked = False
         self.vars = self.witness = None                       # load_circuit: the variable map and the witness buffer
         self.vk = self._vk_transcript = None                  # load_circuit: the verifying key, the transcript after it
@@ -270,13 +276,104 @@ class ResidentProver:
         self.last_challenges = derived
         return proof, pub_int
 
-    def _gather(self, witness_host):
-        """the witness in, the wire and public-input evaluations gathered on the device; returns the public inputs"""
+    def _gather(self, witness_host, inst=None):
+        """the witness in, the wire and public-input evaluations gathered on the device (into inst's buffers, or the single
+        proof's); returns the public inputs"""
+        inst = self._own if inst is None else inst
         self.witness.copy_(witness_host, non_blocking=True)
         self._sync()                                           # torch's stream -> the library's stream
         P = lambda t: t.data_ptr()
-        self.ctx.witness_gather_dev(P(self.witness), self.num_vars, P(self.vars), N_WIRE, self.n, self.num_inputs, P(self.wire_eval), P(self.pub))
-        return self.pub[:self.num_inputs].cpu().numpy().view(np.uint64).copy()
+        self.ctx.witness_gather_dev(P(self.witness), self.num_vars, P(self.vars), N_WIRE, self.n, self.num_inputs, P(inst.wire_eval), P(inst.pub))
+        return inst.pub[:self.num_inputs].cpu().numpy().view(np.uint64).copy()
+
+    # ---- a batch of proofs of one circuit (DESIGN.md 3.11)
+    def instance_bytes(self) -> int:
+        """device memory of one more batch instance: 5 wire evaluations, the public input (n each), 5 wires (n + 2) and z (n + 3)"""
+        n = self.n
+        return 32 * (N_WIRE * n + n + N_WIRE * (n + BLIND_WIRE) + n + BLIND_Z)
+
+    def max_batch(self) -> int:
+        """the largest k prove_batch takes: instance 0 lives in the single proof's buffers, each further one needs
+        instance_bytes(), from the device's free memory (plus what torch caches and the instances already allocated) less
+        one quotient-domain buffer (the final iNTT's scratch) and BATCH_MARGIN_BYTES; never below a batch that has already
+        run (its instances are kept, and the library's pool has grown to serve it).  CPU_MAX_BATCH on the CPU emulator"""
+        if self.dev == "cpu":
+            return self.CPU_MAX_BATCH
+        t = self.torch
+        free, _ = t.cuda.mem_get_info(t.device(self.dev))
+        free += t.cuda.memory_reserved(self.dev) - t.cuda.memory_allocated(self.dev) + len(self._extra) * self.instance_bytes()
+        return 1 + max(len(self._extra), (free - self.m * 32 - self.BATCH_MARGIN_BYTES) // self.instance_bytes())
+
+    def _instances(self, k):
+        """instance 0 and k - 1 resident instances, allocated on first use and kept"""
+        def buf(count):
+            return self.torch.zeros((count, 4), dtype=self.torch.int64, device=self.dev)
+        n = self.n
+        while len(self._extra) < k - 1:
+            self._extra.append(_Instance(buf(N_WIRE * n), buf(n), [buf(n + BLIND_WIRE) for _ in range(N_WIRE)], buf(n + BLIND_Z)))
+        return [self._own] + self._extra[:k - 1]
+
+    def prove_batch(self, witnesses_host, blind=True):
+        """one BatchProof of k = len(witnesses_host) instances of the circuit given to load_circuit (DESIGN.md 3.11): the
+        instances share one transcript, one quotient (sum_i alpha^(3i) Q_i) and one pair of openings.  witnesses_host: k
+        witnesses as in prove_circuit; blind: True (library-drawn scalars), False, or k arrays of shape [13, 4] (one per
+        instance, as prove's).  A batch of one is prove_circuit's proof, call for call.  Returns (BatchProof, [public inputs
+        of each instance as canonical ints]); sets last_challenges and last_transcript_ms as prove_circuit does.
+        ValueError for k = 0, k > max_batch(), or wrong shapes"""
+        from .proof import BatchProof
+        if self._vk_transcript is None:
+            raise ValueError("prove_batch needs a circuit: call load_circuit first")
+        k = len(witnesses_host)
+        if k == 0:
+            raise ValueError("prove_batch needs at least one witness")
+        if k > self.max_batch():
+            raise ValueError(f"a batch of {k} needs {k - 1} x {_gib(self.instance_bytes())} GiB beside the prover: max_batch() = {self.max_batch()}")
+        for i, w in enumerate(witnesses_host):
+            if tuple(w.shape) != (self.num_vars, 4):
+                raise ValueError(f"witness {i}: shape ({self.num_vars}, 4), not {tuple(w.shape)}")
+        if blind is True or blind is False:
+            blinded, scalars = self._blinding(blind)
+            scalars = [scalars] * k
+        else:
+            if len(blind) != k:
+                raise ValueError(f"blind: {len(blind)} blinding arrays for {k} witnesses")
+            if any(b is True or b is False for b in blind):
+                raise ValueError("blind: True, False, or one [13, 4] array per witness")
+            blinded, scalars = True, [self._blinding(b)[1] for b in blind]
+        import time
+        insts = self._instances(k)
+        pubs = [self._gather(w, inst) for w, inst in zip(witnesses_host, insts)]
+        t0 = time.perf_counter()
+        pub_int = [[fr_to_int(v) for v in pub] for pub in pubs]
+        tr = self._vk_transcript.clone()
+        tr.append_pub_input(pub_int[0])
+        for pi in pub_int[1:]:
+            tr.append_vk(self.vk)
+            tr.append_pub_input(pi)
+        clock = [time.perf_counter() - t0]
+
+        def challenges(stage, outputs):
+            t1 = time.perf_counter()
+            if stage == "evals":
+                ev = [fr_to_int(v) for v in outputs]
+                for i in range(0, len(ev), 2 * N_WIRE):
+                    tr.append_proof_evaluations(ev[i:i + N_WIRE], ev[i + N_WIRE:i + 2 * N_WIRE - 1], ev[i + 2 * N_WIRE - 1])
+            else:
+                tr.append_commitments({"wires": b"witness_poly_comms", "perm": b"perm_poly_comms", "quot": b"quot_poly_comms"}[stage],
+                                      [point_from_jacobian(c) for c in outputs])
+            names = {"wires": ("beta", "gamma"), "perm": ("alpha",), "quot": ("zeta",), "evals": ("v",)}[stage]
+            out = {name: fr_from_int(tr.get_and_append_challenge(name.encode())) for name in names}
+            derived.update(out)
+            clock[0] += time.perf_counter() - t1
+            return out
+
+        derived = {}
+        com, evals = self._rounds(challenges, blinded, scalars, insts)
+        t2 = time.perf_counter()
+        proof = BatchProof.from_raw(k, com, evals)
+        self.last_transcript_ms = (clock[0] + time.perf_counter() - t2) * 1e3
+        self.last_challenges = derived
+        return proof, pub_int
 
     def _blinding(self, blind):
         """(blinded, scalars or None) from prove's `blind` argument"""
@@ -290,81 +387,148 @@ class ResidentProver:
                     raise ValueError(f"blind: an array of shape ({N_BLIND}, 4) of raw Fr, True or False, not shape {scalars.shape}")
         return blinded, scalars
 
-    def _rounds(self, challenges, blinded, scalars):
-        """rounds 1-5 from the wire and public-input evaluations in self.wire_eval / self.pub.  challenges(stage, outputs)
-        -> dict of raw Fr challenges, asked where the reference asks its transcript: "wires" (the 5 wire commitments) ->
-        beta, gamma; "perm" ([z's commitment]) -> alpha; "quot" (the 5 quotient-chunk commitments) -> zeta; "evals" (the
-        10 evaluations) -> v"""
-        ctx, n, m, log_n, F = self.ctx, self.n, self.m, self.log_n, self.F
-        log_m = log_n + 3
-        com, P = [], lambda t: t.data_ptr()
-        nw, nz = (n + BLIND_WIRE, n + BLIND_Z) if blinded else (n, n)   # coefficients of each wire / of z
+    def _rounds(self, challenges, blinded, scalars, insts=None):
+        """rounds 1-5 from the wire and public-input evaluations in self.wire_eval / self.pub (insts None), or of the
+        instances of a batch (insts: _Instance list, scalars: one blinding array or None per instance).  challenges(stage,
+        outputs) -> dict of raw Fr challenges, asked where the reference asks its transcript: "wires" (the 5 wire
+        commitments of each instance) -> beta, gamma; "perm" (each instance's commitment of z) -> alpha; "quot" (the 5
+        quotient-chunk commitments) -> zeta; "evals" (the 10 evaluations of each instance) -> v.  Returns (commitments:
+        5k wires, k z, 5 quotient chunks, 2 openings; evaluations: 10 per instance).  A batch of one makes exactly the
+        library calls of a single proof."""
+        if insts is None:
+            insts, scalars = [self._own], [scalars]
+        com = []
+        for inst, sc in zip(insts, scalars):
+            com += self._round1(inst, blinded, sc)
+        ch = dict(challenges("wires", com))
+        for inst, sc in zip(insts, scalars):
+            com.append(self._round2(inst, ch, blinded, sc))
+        ch.update(challenges("perm", com[len(insts) * N_WIRE:]))
+        for inst in insts:
+            self.ctx.ntt_dev(inst.pub.data_ptr(), self.log_n, True, False)
+        com += self._round3(insts, ch, blinded)
+        ch.update(challenges("quot", com[-N_WIRE:]))
+        evals = self._round4(insts, ch, blinded)
+        ch.update(challenges("evals", [v for ev in evals for v in ev]))
+        com += self._round5(insts, ch, blinded, evals)
+        return com, [v for ev in evals for v in ev]
+
+    def _lens(self, blinded):
+        n = self.n
+        return (n + BLIND_WIRE, n + BLIND_Z) if blinded else (n, n)   # coefficients of each wire / of z
+
+    def _round1(self, inst, blinded, scalars):
+        """the wires' coefficient forms (blinded: + (b_0 + b_1 X) Z_H) and their 5 commitments"""
+        ctx, n, log_n, P = self.ctx, self.n, self.log_n, lambda t: t.data_ptr()
+        nw, _ = self._lens(blinded)
         for i in range(N_WIRE):
-            self.wire_coef[i][:n].copy_(self.wire_eval[i * n:(i + 1) * n])
+            inst.wire_coef[i][:n].copy_(inst.wire_eval[i * n:(i + 1) * n])
         if blinded:                                            # the blinding adds to coefficients n, n+1, ...
-            for t in self.wire_coef + [self.z]:
+            for t in inst.wire_coef + [inst.z]:
                 t[n:].zero_()
         self._sync()                                           # torch's stream -> the library's streams
-        # round 1
+        com = []
         for i in range(N_WIRE):
-            ctx.ntt_dev(P(self.wire_coef[i]), log_n, True, False)
+            ctx.ntt_dev(P(inst.wire_coef[i]), log_n, True, False)
             if blinded:
-                ctx.poly_blind_dev(P(self.wire_coef[i]), n, BLIND_WIRE, None if scalars is None else scalars[BLIND_WIRE * i:BLIND_WIRE * (i + 1)])
-            com.append(ctx.commit_dev(P(self.wire_coef[i]), nw))
-        ch = dict(challenges("wires", com[:N_WIRE]))
-        # round 2
-        ctx.perm_product_dev(P(self.wire_eval), P(self.id_eval), P(self.sig_eval), N_WIRE, n, ch["beta"], ch["gamma"], P(self.z))
-        ctx.ntt_dev(P(self.z), log_n, True, False)
+                ctx.poly_blind_dev(P(inst.wire_coef[i]), n, BLIND_WIRE, None if scalars is None else scalars[BLIND_WIRE * i:BLIND_WIRE * (i + 1)])
+            com.append(ctx.commit_dev(P(inst.wire_coef[i]), nw))
+        return com
+
+    def _round2(self, inst, ch, blinded, scalars):
+        """the permutation product z (blinded: + (b_0 + b_1 X + b_2 X^2) Z_H) and its commitment"""
+        ctx, n, P = self.ctx, self.n, lambda t: t.data_ptr()
+        _, nz = self._lens(blinded)
+        ctx.perm_product_dev(P(inst.wire_eval), P(self.id_eval), P(self.sig_eval), N_WIRE, n, ch["beta"], ch["gamma"], P(inst.z))
+        ctx.ntt_dev(P(inst.z), self.log_n, True, False)
         if blinded:
-            ctx.poly_blind_dev(P(self.z), n, BLIND_Z, None if scalars is None else scalars[N_WIRE * BLIND_WIRE:])
-        com.append(ctx.commit_dev(P(self.z), nz))
-        ch.update(challenges("perm", com[N_WIRE:]))
-        ctx.ntt_dev(P(self.pub), log_n, True, False)
-        # round 3: 25 coset evaluations on the 8n domain, the quotient evaluations, one coset-iNTT(8n).  Blinded, the wires
-        # and z are transformed on their first n coefficients and the quotient kernel adds the rest (their tails)
-        srcs = self.sel_coef + self.sig_coef + self.wire_coef + [self.z, self.pub]
+            ctx.poly_blind_dev(P(inst.z), n, BLIND_Z, None if scalars is None else scalars[N_WIRE * BLIND_WIRE:])
+        return ctx.commit_dev(P(inst.z), nz)
+
+    def _alpha_powers(self, alpha, count, step=3):
+        """alpha^(step i), i < count (raw Fr): the weights of the instances of a batch"""
+        F = self.F
+        a3, cur, out = F.pow_u64(alpha, step), F.from_u64(1), []
+        for _ in range(count):
+            out.append(cur)
+            cur = F.mul(cur, a3)
+        return out
+
+    def _round3(self, insts, ch, blinded):
+        """25 coset evaluations on the 8n domain, the quotient evaluations, one coset-iNTT(8n), 5 commitments of the
+        (n+2)-coefficient chunks.  Blinded, the wires and z are transformed on their first n coefficients and the quotient
+        kernel adds the rest (their tails).  A batch: the 18 key polynomials are transformed once (per slice, sliced); each
+        instance i then transforms its 7 and adds alpha^(3i) times its quotient (instance 0 writes it)"""
+        ctx, n, m, P = self.ctx, self.n, self.m, lambda t: t.data_ptr()
+        log_m = self.log_n + 3
+        keys = self.sel_coef + self.sig_coef
+        own = lambda inst: inst.wire_coef + [inst.z, inst.pub]
         qargs = (self.k, ch["alpha"], ch["beta"], ch["gamma"])
-        tails = [(P(t) + 32 * n, BLIND_WIRE) for t in self.wire_coef] + [(P(self.z) + 32 * n, BLIND_Z)] if blinded else None
-        if self.quotient == "whole":   # only the n coefficients at the head of each buffer are read
-            for dst, src in zip(self.big, srcs):
-                dst[:n].copy_(src[:n])
-            self._sync()
-            for dst in self.big:
-                ctx.ntt_dev_padded(P(dst), n, log_m, False, True, wait=False)
-            b = [P(t) for t in self.big]
-            if blinded:
-                ctx.quotient_evals_tail_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, tails, P(self.quot))
+        scale = self._alpha_powers(ch["alpha"], len(insts))
+
+        def tails(inst):
+            return [(P(t) + 32 * n, BLIND_WIRE) for t in inst.wire_coef] + [(P(inst.z) + 32 * n, BLIND_Z)] if blinded else None
+
+        def quotient(b, i, inst, slice_=None):
+            if i:
+                ctx.quotient_evals_acc_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, tails(inst), scale[i], P(self.quot), slice_)
+            elif slice_ is None:
+                if blinded:
+                    ctx.quotient_evals_tail_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, tails(inst), P(self.quot))
+                else:
+                    ctx.quotient_evals_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, P(self.quot))
+            elif blinded:
+                ctx.quotient_evals_slice_tail_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, tails(inst), slice_, P(self.quot))
             else:
-                ctx.quotient_evals_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, P(self.quot))
+                ctx.quotient_evals_slice_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, slice_, P(self.quot))
+
+        if self.quotient == "whole":   # only the n coefficients at the head of each buffer are read
+            b = [P(t) for t in self.big]
+            for i, inst in enumerate(insts):
+                dsts = self.big if i == 0 else self.big[len(keys):]
+                for dst, src in zip(dsts, (keys if i == 0 else []) + own(inst)):
+                    dst[:n].copy_(src[:n])
+                self._sync()                                   # (the previous quotient call has returned: its reads are done)
+                for dst in dsts:
+                    ctx.ntt_dev_padded(P(dst), n, log_m, False, True, wait=False)
+                quotient(b, i, inst)
         else:                          # slice k into the same 25 n-point buffers, every k; all of it on the library's stream
             b = [P(t) for t in self.slices]
             for k in range(m // n):
-                for dst, src in zip(b, srcs):
-                    ctx.ntt_dev_quot_slice(P(src), n, k, dst, wait=False)
-                if blinded:
-                    ctx.quotient_evals_slice_tail_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, tails, k, P(self.quot))
-                else:
-                    ctx.quotient_evals_slice_dev(b[:13], b[13:18], b[18:23], b[23], b[24], *qargs, k, P(self.quot))
+                for i, inst in enumerate(insts):
+                    srcs = (keys if i == 0 else []) + own(inst)
+                    for dst, src in zip(b[len(b) - len(srcs):], srcs):
+                        ctx.ntt_dev_quot_slice(P(src), n, k, dst, wait=False)
+                    quotient(b, i, inst, k)
         ctx.ntt_dev(P(self.quot), log_m, True, True)
         chunk = n + 2
-        for j in range(N_WIRE):
-            com.append(ctx.commit_dev(P(self.quot) + 32 * j * chunk, chunk))
-        ch.update(challenges("quot", com[N_WIRE + 1:]))
-        # round 4
+        return [ctx.commit_dev(P(self.quot) + 32 * j * chunk, chunk) for j in range(N_WIRE)]
+
+    def _round4(self, insts, ch, blinded):
+        """per instance the 5 wires and 4 sigmas at zeta and z at zeta * omega; the sigma values are the same for every
+        instance and are computed once"""
+        ctx, n, P = self.ctx, self.n, lambda t: t.data_ptr()
+        nw, nz = self._lens(blinded)
         zeta = ch["zeta"]
-        zeta_w = F.mul(zeta, F.omega)
-        w_ev = [ctx.poly_eval(P(self.wire_coef[i]), zeta, nw) for i in range(N_WIRE)]
-        s_ev = [ctx.poly_eval(P(self.sig_coef[i]), zeta, n) for i in range(N_WIRE - 1)]
-        z_next = ctx.poly_eval(P(self.z), zeta_w, nz)
-        ch.update(challenges("evals", w_ev + s_ev + [z_next]))
-        # round 5: the scalar coefficients are host glue (a few dozen field operations), the polynomials stay put
+        zeta_w = self.F.mul(zeta, self.F.omega)
+        out, s_ev = [], None
+        for inst in insts:
+            w_ev = [ctx.poly_eval(P(inst.wire_coef[i]), zeta, nw) for i in range(N_WIRE)]
+            if s_ev is None:
+                s_ev = [ctx.poly_eval(P(self.sig_coef[i]), zeta, n) for i in range(N_WIRE - 1)]
+            out.append(w_ev + s_ev + [ctx.poly_eval(P(inst.z), zeta_w, nz)])
+        return out
+
+    def _lin_scalars(self, ev, ch, vanish, lag1):
+        """one instance's linearisation scalars from its 10 evaluations: the 13 selectors', z's and sigma_4's (host glue, a
+        few dozen field operations)"""
+        F = self.F
+        w_ev, s_ev, z_next = ev[:N_WIRE], ev[N_WIRE:2 * N_WIRE - 1], ev[-1]
         a, bb, c, d, e = w_ev
         ab, cd = F.mul(a, bb), F.mul(c, d)
         p5 = lambda x: F.mul(F.mul(F.mul(x, x), F.mul(x, x)), x)
         neg = lambda x: F.sub(F.from_u64(0), x)
-        one = F.from_u64(1)
-        vanish = F.sub(F.pow_u64(zeta, n), one)
-        lag1 = F.mul(vanish, F.inv(F.mul(F.from_u64(n), F.sub(zeta, one))))
+        zeta = ch["zeta"]
         cz = ch["alpha"]
         for wv, kk in zip(w_ev, self.k):
             cz = F.mul(cz, F.add(F.add(wv, F.mul(F.mul(ch["beta"], kk), zeta)), ch["gamma"]))
@@ -373,27 +537,67 @@ class ResidentProver:
         for wv, sv in zip(w_ev[:-1], s_ev):
             cs = F.mul(cs, F.add(F.add(wv, F.mul(ch["beta"], sv)), ch["gamma"]))
         cs = neg(cs)
+        return [a, bb, c, d, ab, cd, p5(a), p5(bb), p5(c), p5(d), neg(e), F.from_u64(1), F.mul(F.mul(ab, cd), e)], cz, cs
+
+    def _round5(self, insts, ch, blinded, evals):
+        """the linearisation polynomial, the batch polynomial at zeta and its opening W, the (batched) z at zeta * omega and
+        its opening W'.  A batch weights instance i's linearisation scalars with alpha^(3i) and its openings with v powers
+        (DESIGN.md 3.11); the polynomials stay put"""
+        ctx, n, F, P = self.ctx, self.n, self.F, lambda t: t.data_ptr()
+        nw, nz = self._lens(blinded)
+        k = len(insts)
+        zeta = ch["zeta"]
+        zeta_w = F.mul(zeta, F.omega)
+        one = F.from_u64(1)
+        vanish = F.sub(F.pow_u64(zeta, n), one)
+        lag1 = F.mul(vanish, F.inv(F.mul(F.from_u64(n), F.sub(zeta, one))))
         zn2 = F.mul(F.add(vanish, one), F.mul(zeta, zeta))
-        qc, cur = [], neg(vanish)
+        qc, cur = [], F.sub(F.from_u64(0), vanish)
         for _ in range(N_WIRE):
             qc.append(cur)
             cur = F.mul(cur, zn2)
-        coeffs = [a, bb, c, d, ab, cd, p5(a), p5(bb), p5(c), p5(d), neg(e), one, F.mul(F.mul(ab, cd), e), cz, cs] + qc
-        polys = [P(t) for t in self.sel_coef] + [P(self.z), P(self.sig_coef[N_WIRE - 1])] + [P(self.quot) + 32 * j * chunk for j in range(N_WIRE)]
-        lens = [n] * N_SEL + [nz, n] + [chunk] * N_WIRE
+        scale = self._alpha_powers(ch["alpha"], k)
+        sel, cz, cs = None, [], None
+        for i, ev in enumerate(evals):
+            q_i, cz_i, cs_i = self._lin_scalars(ev, ch, vanish, lag1)
+            if i:
+                q_i, cz_i, cs_i = [F.mul(scale[i], x) for x in q_i], F.mul(scale[i], cz_i), F.mul(scale[i], cs_i)
+            sel = q_i if sel is None else [F.add(x, y) for x, y in zip(sel, q_i)]
+            cs = cs_i if cs is None else F.add(cs, cs_i)
+            cz.append(cz_i)
+        chunk = n + 2
+        # instance 0's z where the single proof has it, the other instances' z after the quotient chunks
+        coeffs = sel + [cz[0], cs] + qc + cz[1:]
+        polys = [P(t) for t in self.sel_coef] + [P(insts[0].z), P(self.sig_coef[N_WIRE - 1])] + [P(self.quot) + 32 * j * chunk for j in range(N_WIRE)] \
+            + [P(inst.z) for inst in insts[1:]]
+        lens = [n] * N_SEL + [nz, n] + [chunk] * N_WIRE + [nz] * (k - 1)
         lin_len = max(chunk, nz)                               # n + 2, or n + 3 with the blinded z
         ctx.poly_lincomb(polys, np.stack(coeffs), out_len=lin_len, lens=lens, out_ptr=P(self.lin))
-        vs, cur = [], one
-        for _ in range(1 + N_WIRE + N_WIRE - 1):
-            vs.append(cur)
-            cur = F.mul(cur, ch["v"])
-        polys = [P(self.lin)] + [P(t) for t in self.wire_coef] + [P(t) for t in self.sig_coef[:-1]]
-        ctx.poly_lincomb(polys, np.stack(vs), out_len=lin_len, lens=[lin_len] + [nw] * N_WIRE + [n] * (N_WIRE - 1), out_ptr=P(self.batch))
+        vp = self._alpha_powers(ch["v"], 1 + 9 * k, step=1)   # v^(1 + 9i + j): wire j of instance i; v^(6 + 9i + j): sigma j
+        sig_c = [vp[6 + j] for j in range(N_WIRE - 1)]
+        for i in range(1, k):
+            sig_c = [F.add(x, vp[6 + 9 * i + j]) for j, x in enumerate(sig_c)]
+        coeffs = [one] + vp[1:1 + N_WIRE] + sig_c + [vp[1 + 9 * i + j] for i in range(1, k) for j in range(N_WIRE)]
+        polys = [P(self.lin)] + [P(t) for t in insts[0].wire_coef] + [P(t) for t in self.sig_coef[:-1]] \
+            + [P(t) for inst in insts[1:] for t in inst.wire_coef]
+        lens = [lin_len] + [nw] * N_WIRE + [n] * (N_WIRE - 1) + [nw] * (N_WIRE * (k - 1))
+        ctx.poly_lincomb(polys, np.stack(coeffs), out_len=lin_len, lens=lens, out_ptr=P(self.batch))
         ctx.poly_div_linear(P(self.batch), zeta, lin_len, P(self.wit[0]))
-        com.append(ctx.commit_dev(P(self.wit[0]), lin_len - 1))
-        ctx.poly_div_linear(P(self.z), zeta_w, nz, P(self.wit[1]))
+        com = [ctx.commit_dev(P(self.wit[0]), lin_len - 1)]
+        shifted = insts[0].z
+        if k > 1:                                              # sum_i v^i z_i, in the linearisation's buffer (done with)
+            ctx.poly_lincomb([P(inst.z) for inst in insts], np.stack(vp[:k]), out_len=nz, lens=[nz] * k, out_ptr=P(self.lin))
+            shifted = self.lin
+        ctx.poly_div_linear(P(shifted), zeta_w, nz, P(self.wit[1]))
         com.append(ctx.commit_dev(P(self.wit[1]), nz - 1))
-        return com, w_ev + s_ev + [z_next]
+        return com
+
+
+class _Instance:
+    """one instance's resident state: the wire and public-input evaluations, the wires' and z's coefficient forms"""
+
+    def __init__(self, wire_eval, pub, wire_coef, z):
+        self.wire_eval, self.pub, self.wire_coef, self.z = wire_eval, pub, wire_coef, z
 
 
 class NumpyField:

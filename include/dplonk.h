@@ -338,6 +338,17 @@ int dp_quotient_evals_tail_dev(dp_ctx *ctx, const dp_quotient_args *dev_arrays, 
 int dp_quotient_evals_slice_tail_dev(dp_ctx *ctx, const dp_quotient_args *slice_arrays, const dp_quotient_tails *tails,
                                      uint32_t slice, void *out_dev);
 
+/* Round 3 of a batch proof (DESIGN.md 3.11): out_dev[pt] += scale * Q(pt), Q the quotient value the entries above write,
+ * over the whole coset (dev_arrays: 25 arrays of m Fr) or over the points of one slice (slice_arrays: n Fr each; only
+ * out_dev[slice + (m/n) i] is read and written).  The batch quotient sum_i alpha^(3i) Q_i is one call per instance into
+ * the same output, instance 0 through the non-accumulating entries.  tails: as above, or NULL for unblinded wires and z.
+ * scale32: 1 raw Fr below r, host.  The result is byte for byte dp_poly_lincomb_dev([out, Q], [1, scale]).  DP_E_ARG
+ * for a scale not below r, an output that overlaps any of the 25 inputs or a tail; else the errors of the entries above. */
+int dp_quotient_evals_acc_dev(dp_ctx *ctx, const dp_quotient_args *dev_arrays, const dp_quotient_tails *tails, const void *scale32,
+                              void *out_dev);
+int dp_quotient_evals_slice_acc_dev(dp_ctx *ctx, const dp_quotient_args *slice_arrays, const dp_quotient_tails *tails,
+                                    uint32_t slice, const void *scale32, void *out_dev);
+
 /* Blinding, as the reference prover does it to every wire (k = 2) and to z (k = 3): coeffs += b(X) * (X^n - 1),
  * b(X) = b_0 + b_1 X + ... + b_(k-1) X^(k-1), in place on a device buffer of at least n + k Fr (b_j is subtracted
  * from coefficient j and added to coefficient n + j).  blind: k raw Fr below r on the host (reproducible, for
@@ -352,7 +363,9 @@ int dp_poly_eval_dev(dp_ctx *ctx, const void *coeffs_dev, size_t n, const void *
 
 /* Round 5, the folds of src/dispatcher2.rs:566-649 (lin_poly, r_quot, batch_poly):
  * out[j] = sum_{i<k} coeffs[i] * polys[i][j], polys[i] zero-extended past lens[i]; k <= 32.
- * polys / lens / coeffs are host arrays; polys[i] points to host (plain) or device (_dev) memory.  */
+ * polys / lens / coeffs are host arrays; polys[i] points to host (plain) or device (_dev) memory.
+ * The combination is element-wise, so out_dev may be one of the operands (the same pointer, read at j before out[j] is
+ * written): more than 32 operands are chained, out = lincomb(first 32), then out = lincomb([out] + next 31, [1, ...]). */
 int dp_poly_lincomb(dp_ctx *ctx, const void *const *polys, const size_t *lens, const void *coeffs, size_t k, void *out, size_t out_len);
 int dp_poly_lincomb_dev(dp_ctx *ctx, const void *const *polys_dev, const size_t *lens, const void *coeffs, size_t k, void *out_dev,
                         size_t out_len);

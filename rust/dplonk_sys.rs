@@ -84,6 +84,11 @@ extern "C" {
                                       out_dev: *mut c_void) -> c_int;
     pub fn dp_quotient_evals_slice_tail_dev(ctx: *mut dp_ctx, slice_arrays: *const dp_quotient_args, tails: *const dp_quotient_tails,
                                             slice: u32, out_dev: *mut c_void) -> c_int;
+    /// out_dev += scale * quotient: round 3 of a batch proof; tails may be null (unblinded)
+    pub fn dp_quotient_evals_acc_dev(ctx: *mut dp_ctx, dev_arrays: *const dp_quotient_args, tails: *const dp_quotient_tails,
+                                     scale_fr: *const u8, out_dev: *mut c_void) -> c_int;
+    pub fn dp_quotient_evals_slice_acc_dev(ctx: *mut dp_ctx, slice_arrays: *const dp_quotient_args, tails: *const dp_quotient_tails,
+                                           slice: u32, scale_fr: *const u8, out_dev: *mut c_void) -> c_int;
     pub fn dp_poly_blind_dev(ctx: *mut dp_ctx, coeffs_dev: *mut c_void, n: usize, k: u32, blind_kfr: *const u8) -> c_int;
     pub fn dp_wire_permutation_scratch_bytes(num_wire_types: usize, n: usize, num_vars: u64, bytes: *mut usize) -> c_int;
     pub fn dp_wire_permutation_dev(ctx: *mut dp_ctx, vars_dev: *const u32, num_wire_types: usize, n: usize, num_vars: u64,
